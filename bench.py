@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — frames/sec of the per-frame perception hot path (BASELINE.json metric) on N B200s.
+"""bench.py — frames/sec of the per-frame perception hot path (BASELINE.json metric) on N H100s.
 
 Default workload (`--workload c2`, BASELINE.json configs[1]): PointPillars + PyramidFusion (`heter_pyramid_collab`, yaml
 m1_pyramid), 5 agents, 64-line synthetic LiDAR scene, range +-102.4 m -> 512x512 pillars, fusion at 256x256.  A step = one
@@ -8,7 +8,7 @@ deblocks -> shrink -> cls/reg/dir heads.  `--workload c1|c3|c4|c5` run the other
 
   value         frames/s with the (already uploaded) point clouds resident in HBM, one CUDA-event interval over K frames
   e2e           frames/s through the serving entry point with HOST (pinned) inputs: H2D + frame + D2H of the predictions
-  roofline      dominant kernel (tcgen05 conv) vs the measured tensor peak + `kernels[]`: every named op with its algorithmic
+  roofline      dominant kernel (wgmma conv) vs the measured tensor peak + `kernels[]`: every named op with its algorithmic
                 bytes / FLOPs (SURVEY.md 8d), live CUDA-event time, achieved GB/s and TFLOP/s and the fraction of its roof
   parity        max |GPU - reference| per head on a FULL-SIZE frame of this workload (the frame the cpu_baseline leg computes);
                 the process exits non-zero when it is above the tolerance (1e-3 tc32/fp32, 1e-2 bf16, relative to max(1,|ref|))
@@ -190,8 +190,8 @@ def pick_host_threads():
 
 
 PRECISION_TEXT = {
-    "tc32": "fp32-equivalent: split-bf16 operands (hi+lo planes), 3 tcgen05 MMAs per K-step (2 for N<=64), fp32 accumulate in TMEM",
-    "bf16": "bf16 operands on tcgen05, fp32 accumulate",
+    "tc32": "fp32-equivalent: split-bf16 operands (hi+lo planes), 3 wgmma per K-step (2 for N<=64), fp32 accumulate in registers",
+    "bf16": "bf16 operands on wgmma, fp32 accumulate",
     "fp32": "fp32 storage, fp32 FMA on CUDA cores",
 }
 
@@ -207,7 +207,7 @@ def queue_ahead(ms=40.0):
 def workload_config(workload, n_gpus, parallelism, precision=None):
     cfg = {"workload": wcfg.WORKLOADS[workload]["title"],
            "parallelism": parallelism if n_gpus > 1 else "single-gpu",
-           "l2_policy": "per-frame working set (~1.5 GB activations) >> 126 MB L2; scenes rotate so no frame reuses inputs",
+           "l2_policy": "per-frame working set (~1.5 GB activations) >> the H100 50 MB L2; scenes rotate so no frame reuses inputs",
            "launch": "one CUDA graph replay per frame (kernels captured once; per-kernel roofline numbers come from an eager, "
                      "event-instrumented pass)"}
     if precision is not None:
@@ -338,6 +338,46 @@ def run_reference(opt):
 # GPU arm
 # ------------------------------------------------------------------------------------------------------------------
 HEADS = ("cls_preds", "reg_preds", "dir_preds")
+# fallback peaks when MEASURED_PEAKS.json is absent: NVIDIA's H100 SXM data sheet (700 W), not measured rates
+H100_HBM_GBS = 3350.0
+H100_BF16_TFLOPS = 989.0
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, outs):
+    """Write the arrays a caller of the timed path receives (one frame) as <name>.npy, float32 (float64 stays float64).
+    An array that would take the total past 64 MiB is replaced by a fixed, seeded sample of its flattened elements
+    (<name>.npy) plus the sampled flat indices (<name>.index.npy)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    flat = {}
+
+    def walk(prefix, v):
+        if isinstance(v, torch.Tensor):
+            flat[prefix] = v
+        elif isinstance(v, dict):
+            for k in sorted(v):
+                walk(f"{prefix}.{k}" if prefix else str(k), v[k])
+        elif isinstance(v, (list, tuple)):
+            for i, x in enumerate(v):
+                walk(f"{prefix}.{i}", x)
+    walk("", outs)
+    budget = DUMP_LIMIT_BYTES
+    rng = np.random.default_rng(0)
+    written = {}
+    for name in sorted(flat):
+        a = flat[name].detach().float().cpu().numpy() if flat[name].dtype != torch.float64 else flat[name].detach().cpu().numpy()
+        if a.nbytes > budget // 2:
+            n = max(1, budget // 2 // (a.itemsize + 8))
+            idx = np.sort(rng.choice(a.size, size=min(n, a.size), replace=False)).astype(np.int64)
+            np.save(os.path.join(out_dir, f"{name}.index.npy"), idx)
+            a = a.reshape(-1)[idx]
+            budget -= idx.nbytes
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+        budget -= a.nbytes
+        written[name] = list(a.shape)
+    return written
 
 
 def parity_record(gpu_out, ref_out, precision, what):
@@ -366,8 +406,8 @@ def parity_record(gpu_out, ref_out, precision, what):
 
 def aggregate_profile(recs, frames, peaks):
     """recs: ops.PROFILE entries (name, flops|callable, ev0, ev1, bytes|callable) of `frames` instrumented frames."""
-    hbm = peaks.get("hbm_gbs", 6577.0)
-    tf = peaks.get("bf16_tflops_sustained", 1400.0)
+    hbm = peaks.get("hbm_gbs", H100_HBM_GBS)
+    tf = peaks.get("bf16_tflops_sustained", H100_BF16_TFLOPS)
     agg = {}
     for name, flops, a, b, nbytes, *_ in recs:
         fl = float(flops() if callable(flops) else flops)
@@ -572,6 +612,9 @@ def main():
     ap.add_argument("--inflight", type=int, default=2, help="captured frames in flight for `value` (N graphs on N streams, heal_b200.graph.FrameInterleaver); 1 = strictly one frame after the other (the number reported as `latency`)")
     ap.add_argument("--pipeline-depth", type=int, default=2, help="e2e: captured frames in flight in FramePipeline (results are delivered depth-1 submits later)")
     ap.add_argument("--no-pipeline", action="store_true", help="e2e: one stream, H2D -> frame -> D2H back to back (no copy/compute overlap)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last step of the serial timed loop (the one reported as latency; the same frames "
+                         "and function as the in-flight loop behind `value`) as DIR/<name>.npy, float32, <= 64 MiB in all")
     opt = ap.parse_args()
     ref = opt.impl == "reference"
     opt.steps = opt.steps if opt.steps is not None else (5 if ref else 20)
@@ -677,7 +720,14 @@ def run_gpu(opt):
             sampler.start()
         # ---- timed region: K frames, ONE device-event interval, inputs resident in HBM ----
         l0 = lib.heal_launch_count()
-        serial_ms = time_frames(frame_dev, opt.steps, barrier)
+        last = {}
+
+        def frame_timed(i):
+            last["out"] = frame_dev(i)
+        serial_ms = time_frames(frame_timed, opt.steps, barrier)
+        if opt.dump_outputs and rank == 0:
+            # the graph's output buffers still hold the last timed frame: copy them out before anything else runs
+            dump_outputs(opt.dump_outputs, last["out"])
         total_ms = serial_ms
         inflight = 1
         if fg is not None and opt.inflight > 1:
@@ -786,9 +836,10 @@ def run_gpu(opt):
 
     rc = 0
     if rank == 0:
-        hbm_peak = peaks.get("hbm_gbs", 6577.0)
-        peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)
-        peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)" if peaks else "fallback 1.4 PFLOP/s sustained"
+        hbm_peak = peaks.get("hbm_gbs", H100_HBM_GBS)
+        peak_tf = peaks.get("bf16_tflops_sustained", H100_BF16_TFLOPS)
+        peak_src = ("MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)" if peaks else
+                    "H100 SXM data sheet, dense BF16 at 700 W (not a measured rate)")
         roofline = None
         if kernels:
             fam = [k for k in kernels if k.startswith("conv_tc")] or [k for k in kernels if k.startswith("conv_")]
@@ -801,7 +852,7 @@ def run_gpu(opt):
             mma_per_flop = 3 if (opt.precision == "tc32" and tc) else 1
             tj, tname = load_ncu_traffic()
             traffic = tj.get("k_conv2d_tc_bytes_per_launch") if tc else None
-            roofline = {"bound": "tensor", "kernel": "k_conv2d_tc + k_gconv3x3_ring (tcgen05 implicit-GEMM conv: 1x1/3x3/grouped/strided/transposed)"
+            roofline = {"bound": "tensor", "kernel": "k_conv2d_tc + k_gconv3x3_ring (wgmma implicit-GEMM conv: 1x1/3x3/grouped/strided/transposed)"
                         if tc else "k_conv2d_dense/grouped (fp32 CUDA cores)",
                         "achieved": ach, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach / peak_tf if ach else None,
                         "traffic": traffic, "traffic_source": f"profiles/{tname}" if traffic else None, "peak_source": peak_src,

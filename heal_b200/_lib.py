@@ -79,7 +79,7 @@ ERRORS = {-1: "HEAL_ERR_ARG", -2: "HEAL_ERR_WORKSPACE", -3: "HEAL_ERR_LAUNCH", -
 def _load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
-            f"{LIB_PATH} not found: build it with `python -m heal_b200.build` (nvcc, sm_100a). "
+            f"{LIB_PATH} not found: build it with `python -m heal_b200.build` (nvcc, sm_90a). "
             "heal_b200 has no CPU / PyTorch fallback.")
     lib = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():

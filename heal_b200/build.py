@@ -1,4 +1,4 @@
-"""Build the C-ABI shared library (libheal_b200.so) in-tree with nvcc for sm_100a.
+"""Build the C-ABI shared library (libheal_b200.so) in-tree with nvcc for sm_90a.
 
 Cross-compiles without a GPU.  `python -m heal_b200.build` or `__graft_entry__.build()`.
 """
@@ -13,7 +13,7 @@ LIB = os.path.join(HERE, "libheal_b200.so")
 STAMP = os.path.join(HERE, "csrc", ".build_stamp")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
 
@@ -59,7 +59,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             sys.stderr.write(f"[heal_b200.build] {src}\n{out}\n")
     if failed:
         raise RuntimeError("nvcc failed")
-    cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB] + objs + ["-lcudart"]
+    cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", LIB] + objs + ["-lcudart"]
     subprocess.check_call(cmd)
     with open(STAMP, "w") as fh:
         fh.write(dig)

@@ -9,7 +9,7 @@ extern "C" int heal_device_check(void) {
     if (cudaGetDevice(&dev) != cudaSuccess) return HEAL_ERR_DRIVER;
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess) return HEAL_ERR_DRIVER;
-    return (prop.major == 10) ? HEAL_OK : HEAL_ERR_UNSUPPORTED;
+    return (prop.major == 9) ? HEAL_OK : HEAL_ERR_UNSUPPORTED;
 }
 
 #include <atomic>

@@ -1,4 +1,4 @@
-// Common device/host helpers for the heal_b200 sm_100a kernels.
+// Common device/host helpers for the heal_b200 sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -12,7 +12,7 @@
 #define HEAL_ERR_UNSUPPORTED (-4)
 #define HEAL_ERR_DRIVER (-5)
 
-#define HEAL_NUM_SMS 148  // B200: 2 dies x 74 SMs
+#define HEAL_NUM_SMS 132  // H100 SXM
 
 // process-wide count of kernels this library has launched (bench.py reports it as gpu_launches)
 extern "C" void heal_launch_counter_add(int n);

@@ -1,5 +1,5 @@
 // fp32 channels-last (NHWC) 2-D convolution on the CUDA cores: the exact-fp32 companion of the
-// tcgen05 implicit-GEMM engine (conv2d_tc.cu). It serves (a) shapes the tensor-core engine does not
+// wgmma implicit-GEMM engine (conv2d_tc.cu). It serves (a) shapes the tensor-core engine does not
 // take (grouped 3x3 with 4-16 channels per group, Cin/Cout not multiples of 16, the 20-channel heads)
 // and (b) as the on-device fp32 cross-check for the tensor-core path in tests.
 // Reference ops replaced: nn.Conv2d / nn.ConvTranspose2d(k == stride) + eval BatchNorm2d (folded on the

@@ -1,4 +1,4 @@
-// Implicit-GEMM 2-D convolution on the 5th-generation tensor cores (tcgen05.mma, accumulators in TMEM),
+// Implicit-GEMM 2-D convolution on the Hopper tensor cores (wgmma.mma_async, fp32 accumulators in registers),
 // operands staged by TMA (cp.async.bulk.tensor) with the 128-byte swizzle, warp-specialised and persistent.
 //
 // Replaces the dense convolutions of the BEV backbones / ResNeXt pyramid / shrink header
@@ -7,7 +7,7 @@
 //
 // Precision ("split-bf16", fp32-equivalent): an fp32 value x is stored as two bf16 planes hi = bf16(x),
 // lo = bf16(x - hi) (16 mantissa bits).  A product a*b is evaluated as a_hi*b_hi + a_hi*b_lo + a_lo*b_hi
-// with fp32 accumulation in TMEM: three tcgen05.mma per K step into the same accumulator, relative
+// with fp32 accumulation: three wgmma per K step into the same accumulator, relative
 // error ~2^-16 per product, which keeps 70 stacked layers inside the 1e-3 fp32 parity tolerance that plain
 // bf16 / tf32 tensor-core math cannot meet.  With planes == 1 the same kernel is a plain bf16 conv.
 //
@@ -17,11 +17,12 @@
 // by the TMA unit, which implements the convolution padding.  B tiles come from the packed weights
 // {Cin, taps*CoutPad, plane}.
 //
-// Roles (320 threads): warp 0 = TMA producer, warp 1 = MMA issuer + TMEM allocator (both loop as converged warps and issue
-// under elect.sync so the tcgen05 / TMA instructions stay on the uniform datapath), warps 2..9 = epilogue, two warps per
-// TMEM lane quarter (TMEM -> registers -> bias / residual / ReLU -> hi/lo split -> swizzled smem staging -> one
-// cp.async.bulk.tensor store per 64-channel chunk; fp32 / transposed-conv outputs use direct stores).
-// Two TMEM accumulator buffers let the epilogue of tile i overlap the MMAs of tile i+1.
+// Roles (384 threads): warpgroup 0 = TMA producer (warp 0 loops as a converged warp and issues under elect.sync; its
+// registers are handed to the consumers with setmaxnreg), warpgroups 1 and 2 = consumers: each runs the M = 64 wgmma of one
+// half of the 128-pixel tile, then both drain the tile together: accumulator chunk -> fp32 scratch in shared memory (rows
+// transposed from the wgmma fragment to one pixel per thread) -> bias / residual / ReLU -> hi/lo split -> swizzled smem
+// staging -> one cp.async.bulk.tensor store per 64-channel chunk (fp32 / transposed-conv outputs use direct stores).
+// The producer keeps STAGES k-blocks in flight, so the next tile's operands arrive while the consumers run the epilogue.
 // Modes: stride 2 through TMA element strides; grouped 3x3 as 16-channel sub-block MMAs on block-diagonal 64-channel
 // tiles; "halo" (3x3, stride 1, one-row tiles, N = 64): one activation box of TW+2 pixels per kernel ROW, the three
 // horizontal taps are row-shifted descriptors of the same smem tile (3x less L2->smem activation traffic).
@@ -35,7 +36,7 @@
 
 namespace {
 
-constexpr int TC_THREADS = 320;      // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue (2 per TMEM lane quarter)
+constexpr int TC_THREADS = 384;      // warpgroup 0 TMA (warp 0), warpgroups 1 and 2 wgmma + epilogue
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;                 // bf16 elements = 128 B = one swizzle row
 constexpr int A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;   // 16 KiB per plane
@@ -78,10 +79,10 @@ template <int BLOCK_N, int STAGES, int STG, bool GELU = false>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
             const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR, const TcP p) {
-    // 1024 B alignment for the 128B swizzle atoms: requested from the toolchain (no slack bytes to round up inside -- the halo +
-    // two-staging-buffer configuration needs all 227 KiB) and checked once.  The pointer is laundered through an empty asm so
-    // that shared-memory addresses stay run-time values: with compile-time-constant addresses ptxas emits a slower kernel
-    // (measured A/B on one box: level-0 1x1 conv 51 -> 66 us).
+    // 1024 B alignment for the 128B swizzle atoms: requested from the toolchain (no slack bytes to round up inside -- the halo
+    // configuration needs all 227 KiB) and checked once.  The pointer is laundered through an empty asm so
+    // that shared-memory addresses stay run-time values: with compile-time-constant addresses ptxas emitted a slower kernel
+    // (an A/B on the B200 build).
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uintptr_t raw_addr = reinterpret_cast<uintptr_t>(smem_raw);
     asm volatile("" : "+l"(raw_addr));
@@ -95,39 +96,30 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     const int stage_bytes = p.halo ? (halo_a_bytes + p.wplanes * 3 * B_TILE_BYTES) : (p.planes * A_TILE_BYTES + p.wplanes * B_TILE_BYTES);
     const int stg_bytes = p.planes * A_TILE_BYTES;                        // one staging buffer: [plane][128 rows][128 B]
     uint8_t* stg = smem + (size_t)STAGES * stage_bytes;                   // 1024-aligned (stage_bytes is a multiple of 1024)
-    uint64_t* bars = reinterpret_cast<uint64_t*>(stg + (size_t)STG * stg_bytes);
-    // bars: full[STAGES], empty[STAGES], tmem_full[2], tmem_empty[2], (spare), residual_full[3]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 8);
-    const uint32_t bar_res = smem_u32(bars + 2 * STAGES + 5);
+    constexpr int SW = BLOCK_N < 64 ? BLOCK_N : 64;                       // accumulator columns per pass through the scratch
+    const uint32_t scr = smem_u32(stg + (size_t)STG * stg_bytes);         // fp32 scratch [128 rows][SW]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(stg + (size_t)STG * stg_bytes + BLOCK_M * SW * 4);
+    // bars: full[STAGES], empty[STAGES], residual_full[3]
+    const uint32_t bar_res = smem_u32(bars + 2 * STAGES);
     const uint32_t smem_base = smem_u32(smem);
     const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + STAGES);
-    const uint32_t bar_tfull = smem_u32(bars + 2 * STAGES), bar_tempty = smem_u32(bars + 2 * STAGES + 2);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // Split-bf16 products a_hi*b_hi + a_hi*b_lo + a_lo*b_hi.  For BLOCK_N <= 64 the hi and lo weight planes sit next to each other
     // in shared memory, so ONE MMA with N' = 2N computes a_hi x [b_hi | b_lo] (main | aux accumulator columns) and a second
-    // N-wide MMA adds a_lo x b_hi: 2 tensor-core instructions and 2 reads of the A slice per K step instead of 3 (these tile
-    // shapes are bound by the A-operand shared-memory reads: a 128x16 N=16 MMA costs ~2/3 of an N=128 one).  The epilogue
-    // adds aux to main.  BLOCK_N = 128 keeps 3 MMAs (N' = 256 would be the same tensor time and needs all of TMEM).
+    // N-wide MMA adds a_lo x b_hi: 2 tensor-core instructions and 2 reads of the A slice per K step instead of 3.  The
+    // consumers add aux to main before the epilogue.  BLOCK_N = 128 keeps 3 MMAs (N' = 256 would need 128 accumulator
+    // registers per thread).
     constexpr bool NCAT = (BLOCK_N <= 64);
-    constexpr int ACC_STRIDE = NCAT ? 2 * BLOCK_N : BLOCK_N;      // TMEM columns per accumulator buffer
-    constexpr int TMEM_COLS = (2 * ACC_STRIDE < 32) ? 32 : 2 * ACC_STRIDE;
+    constexpr int NACC = NCAT ? 2 * BLOCK_N : BLOCK_N;            // accumulator columns per tile half
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(bar_tfull + 8 * a, 1); mbar_init(bar_tempty + 8 * a, 256); }
+        for (int s = 0; s < STAGES; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 8); }   // 8 consumer warps
         for (int a = 0; a < 3; ++a) mbar_init(bar_res + 8 * a, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    // Programmatic dependent launch: everything above (barrier init, TMEM allocation) overlapped the tail of the previous
+    // Programmatic dependent launch: everything above (barrier init) overlapped the tail of the previous
     // kernel in the stream / graph; from here on we touch memory it produced, so wait for it, and let the next kernel start
     // its own prologue as soon as our CTAs begin to drain.
     if (p.pdl) {
@@ -139,9 +131,10 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     const int kcn = p.blockdiag ? 1 : p.kc_blocks;      // channel blocks per tap visited by one tile
     const int kblocks = (p.halo ? 3 : p.taps) * kcn;    // halo mode: one k-block per kernel ROW (3 taps each)
 
-    if (warp == 0) {
-        // ============================== TMA producer (whole warp loops, one elected lane issues) ==
-        {
+    if (warp < 4) {
+        regs_dec<40>();
+        // ============================== TMA producer: warp 0 (whole warp loops, one elected lane issues) ==
+        if (warp == 0) {
             int stage = 0; uint32_t phase = 0;
             for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
                 const int nt = tile % p.n_tiles, mt = tile / p.n_tiles;
@@ -182,129 +175,114 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                 }
             }
         }
-    } else if (warp == 1) {
-        // ============================== MMA issuer (whole warp loops, one elected lane issues) ====
-        {
-            // instruction descriptor: D=f32, A=B=bf16, K-major both, N>>3 @17, M>>4 @24
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BLOCK_N >> 3) << 17) | ((uint32_t)(BLOCK_M >> 4) << 24);
-            const uint32_t idesc16 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(16 >> 3) << 17) | ((uint32_t)(BLOCK_M >> 4) << 24);
-            // N-concatenated forms (NCAT): N' = 2N
-            const uint32_t idesc_cat = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)((2 * BLOCK_N) >> 3) << 17) | ((uint32_t)(BLOCK_M >> 4) << 24);
-            const uint32_t idesc32 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(32 >> 3) << 17) | ((uint32_t)(BLOCK_M >> 4) << 24);
-            const bool split = (p.planes == 2);                      // activations carry a lo plane
-            const bool wsplit = (p.wplanes == 2);                    // weights carry a lo plane
-            const int sub_cols = (NCAT && wsplit) ? 32 : 16;         // accumulator columns per 16-channel diagonal sub-block
-            const int sub_bytes = p.wplanes * 2048;                  // smem bytes per sub-block: [plane][16 rows][128 B]
-            int stage = 0; uint32_t phase = 0;
-            int acc = 0; uint32_t acc_phase = 0;
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-                mbar_wait(bar_tempty + 8 * acc, acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + (uint32_t)(acc * ACC_STRIDE);
-                for (int kb = 0; kb < kblocks; ++kb) {
-                    mbar_wait(bar_full + 8 * stage, phase);
-                    tc_fence_after();
-                    // A: [plane][rows][128 B]; halo mode: tap s reads rows [s, s+128) of the (TW+2)-row tile (start address + s*128 B;
-                    // the swizzle is a function of the absolute smem address, so no base offset)
-                    const uint32_t sa = smem_base + stage * stage_bytes;
-                    const uint32_t a_plane = p.halo ? (uint32_t)halo_a_plane : (uint32_t)A_TILE_BYTES;
-                    const uint32_t sb = sa + (p.halo ? (uint32_t)halo_a_bytes : (uint32_t)(p.planes * A_TILE_BYTES));
-                    const int ntap = p.halo ? 3 : 1;
-                    if (elect_one()) {
-                        if (!(p.dbg & 16))
-                        for (int s = 0; s < ntap; ++s) {
-                            const uint32_t ah = sa + s * 128, al = ah + a_plane;
-                            const uint32_t bs = sb + s * p.wplanes * B_TILE_BYTES;
+    } else {
+        // ============================== consumers (warpgroups 1 and 2): wgmma, then the epilogue ==
+        regs_inc<232>();
+        const int wg = (warp >> 2) - 1;                 // MMAs: tile rows [64 wg, 64 wg + 64)
+        const int quarter = warp & 3;
+        const int chalf = (warp - 4) >> 2;              // epilogue: which half of the tile's column chunks this warp drains
+        const int row = quarter * 32 + lane;            // epilogue: accumulator row = pixel within the tile
+        constexpr int CHUNK = (BLOCK_N >= 32) ? 32 : 16;
+        int stg_count = 0;
+        const bool split = (p.planes == 2);                      // activations carry a lo plane
+        const bool wsplit = (p.wplanes == 2);                    // weights carry a lo plane
+        const int sub_bytes = p.wplanes * 2048;                  // smem bytes per 16-channel diagonal sub-block: [plane][16 rows][128 B]
+        const uint32_t a_plane = p.halo ? (uint32_t)halo_a_plane : (uint32_t)A_TILE_BYTES;
+        const int ntap = p.halo ? 3 : 1;
+        int stage = 0; uint32_t phase = 0;
+        float d[NACC / 2];
 #pragma unroll
-                            for (int k = 0; k < BLOCK_K / 16; ++k) {
-                                const uint64_t a_hi = umma_desc_sw128_off(ah + k * 32, p.bo_mode), a_lo = umma_desc_sw128_off(al + k * 32, p.bo_mode);
-                                if (p.blockdiag) {
-                                    // Grouped conv: channels-per-group divides 16, so output channels [16k,16k+16) of this 64-block depend
-                                    // only on input channels [16k,16k+16): one M128 x N16 x K16 product per 16-channel sub-block.
-                                    // sub-block k: [plane][16 rows] of 128 B rows at K offset k*16 elements, or packed 32 B rows
-                                    const uint32_t bk = p.bdiag ? bs + k * p.wplanes * 512 : bs + k * sub_bytes + k * 32;
-                                    const uint64_t bd = p.bdiag ? umma_desc_sw32(bk) : umma_desc_sw128(bk);
-                                    const uint32_t td = tmem_d + (uint32_t)(k * sub_cols);
-                                    const uint32_t f0 = (kb == 0 && s == 0) ? 0u : 1u;
-                                    if constexpr (NCAT) {
-                                        if (wsplit) {
-                                            umma_bf16(td, a_hi, bd, idesc32, f0);                 // [a_hi*b_hi | a_hi*b_lo]
-                                            if (split) umma_bf16(td, a_lo, bd, idesc16, 1u);      // += a_lo*b_hi
-                                        } else {
-                                            umma_bf16(td, a_hi, bd, idesc16, f0);
-                                        }
-                                    }
+        for (int i = 0; i < NACC / 2; ++i) d[i] = 0.f;
+        // All k-blocks of one tile into d (this warpgroup's 64 rows); afterwards d[0, BLOCK_N / 2) is the fragment of the
+        // BLOCK_N logical columns (main + aux folded).
+        auto mma_tile = [&]() {
+            int prev = -1;
+            for (int kb = 0; kb < kblocks; ++kb) {
+                mbar_wait(bar_full + 8 * stage, phase);
+                // A: [plane][rows][128 B]; halo mode: tap s reads rows [s, s+128) of the (TW+2)-row tile (start address + s*128 B)
+                const uint32_t sa = smem_base + stage * stage_bytes;
+                const uint32_t sb = sa + (p.halo ? (uint32_t)halo_a_bytes : (uint32_t)(p.planes * A_TILE_BYTES));
+                wgmma_fence();
+                if (!(p.dbg & 16))
+                for (int s = 0; s < ntap; ++s) {
+                    const uint32_t ah = sa + (uint32_t)(wg * 64 * 128 + s * 128), al = ah + a_plane;
+                    const uint32_t bs = sb + s * p.wplanes * B_TILE_BYTES;
+#pragma unroll
+                    for (int k = 0; k < BLOCK_K / 16; ++k) {
+                        const uint64_t a_hi = gmma_desc_sw128_off(ah + k * 32, p.bo_mode), a_lo = gmma_desc_sw128_off(al + k * 32, p.bo_mode);
+                        if (p.blockdiag) {
+                            if constexpr (BLOCK_N == 64) {
+                                // Grouped conv: channels-per-group divides 16, so output channels [16k,16k+16) of this 64-block depend
+                                // only on input channels [16k,16k+16): one M64 x N16 x K16 product per 16-channel sub-block, into
+                                // its own accumulator registers d[16k ..] ([main16 | aux16]) or d[8k ..].
+                                // sub-block k: [plane][16 rows] of 128 B rows at K offset k*16 elements, or packed 32 B rows
+                                const uint32_t bk = p.bdiag ? bs + k * p.wplanes * 512 : bs + k * sub_bytes + k * 32;
+                                const uint64_t bd = p.bdiag ? gmma_desc_sw32(bk) : gmma_desc_sw128(bk);
+                                const uint32_t f0 = (kb == 0 && s == 0) ? 0u : 1u;
+                                if (wsplit) {
+                                    wgmma_bf16<32>(d + 16 * k, a_hi, bd, f0);               // [a_hi*b_hi | a_hi*b_lo]
+                                    if (split) wgmma_bf16<16>(d + 16 * k, a_lo, bd, 1u);    // += a_lo*b_hi
                                 } else {
-                                    const uint32_t first = (kb == 0 && s == 0 && k == 0) ? 0u : 1u;
-                                    const uint64_t b_hi = umma_desc_sw128(bs + k * 32);
-                                    if (!wsplit) {
-                                        umma_bf16(tmem_d, a_hi, b_hi, idesc, first);
-                                    } else if constexpr (NCAT) {
-                                        umma_bf16(tmem_d, a_hi, b_hi, idesc_cat, first);                // [a_hi*b_hi | a_hi*b_lo]
-                                        if (split) umma_bf16(tmem_d, a_lo, b_hi, idesc, 1u);            // += a_lo*b_hi
-                                    } else {
-                                        const uint64_t b_lo = umma_desc_sw128(bs + B_TILE_BYTES + k * 32);
-                                        umma_bf16(tmem_d, a_hi, b_lo, idesc, first);
-                                        if (split) umma_bf16(tmem_d, a_lo, b_hi, idesc, 1u);
-                                        umma_bf16(tmem_d, a_hi, b_hi, idesc, 1u);
-                                    }
+                                    wgmma_bf16<16>(d + 8 * k, a_hi, bd, f0);
                                 }
                             }
+                        } else {
+                            const uint32_t first = (kb == 0 && s == 0 && k == 0) ? 0u : 1u;
+                            const uint64_t b_hi = gmma_desc_sw128(bs + k * 32);
+                            if (!wsplit) {
+                                wgmma_bf16<BLOCK_N>(d, a_hi, b_hi, first);
+                            } else if constexpr (NCAT) {
+                                wgmma_bf16<2 * BLOCK_N>(d, a_hi, b_hi, first);               // [a_hi*b_hi | a_hi*b_lo]
+                                if (split) wgmma_bf16<BLOCK_N>(d, a_lo, b_hi, 1u);           // += a_lo*b_hi
+                            } else {
+                                const uint64_t b_lo = gmma_desc_sw128(bs + B_TILE_BYTES + k * 32);
+                                wgmma_bf16<BLOCK_N>(d, a_hi, b_lo, first);
+                                if (split) wgmma_bf16<BLOCK_N>(d, a_lo, b_hi, 1u);
+                                wgmma_bf16<BLOCK_N>(d, a_hi, b_hi, 1u);
+                            }
                         }
-                        umma_commit(bar_empty + 8 * stage);       // smem slot free once these MMAs retire
                     }
-                    __syncwarp();
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
-                if (elect_one()) umma_commit(bar_tfull + 8 * acc);   // accumulator ready for the epilogue
-                __syncwarp();
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+                wgmma_commit();
+                wgmma_wait<1>();                                   // the previous k-block's MMAs have retired: free its stage
+                if (prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev);
+                prev = stage;
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
             }
-        }
-    } else {
-        // ============================== epilogue (warps 2..5) =====================
-        const int quarter = warp & 3;                   // TMEM lane quarter this warp may access
-        const int chalf = (warp - 2) >> 2;              // which half of the tile's column chunks this warp drains
-        const int row = quarter * 32 + lane;            // accumulator row = pixel within the tile
-        constexpr int CHUNK = (BLOCK_N >= 32) ? 32 : 16;
-        int acc = 0; uint32_t acc_phase = 0;
-        int stg_count = 0;
-        // Residual prefetch (TMA-store epilogue, split/bf16 residual): the 2 x 4 x 16 B of this thread's row for the NEXT 64-channel
-        // chunk are requested one chunk ahead, so their DRAM latency hides behind the current chunk (and the wait for the MMAs)
-        // instead of stalling every 8-channel group (measured: level-0 conv3 105 -> 44 us with the loads removed).
-        // CH logical accumulator columns [col0, col0+CH) of buffer `acc` -> raw (fp32 bits); with the N-concatenated split MMAs the
-        // value is main + aux: dense = columns c and BLOCK_N + c, block-diagonal = per 16-channel sub-block [main16 | aux16].
-        auto ld_acc = [&](int col0, uint32_t* raw) {
-            const uint32_t tb = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * ACC_STRIDE);
-            if (NCAT && p.wplanes == 2) {
-                uint32_t y[CHUNK];
-                if constexpr (CHUNK == 32) {
-                    if (p.blockdiag) {
-                        tmem_ld32(tb + (uint32_t)(2 * col0), raw); tmem_ld32(tb + (uint32_t)(2 * col0 + 32), y);
-                        tmem_wait_ld();
+            wgmma_wait<0>();
+            if (prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev);
+            if constexpr (NCAT) {
+                if (wsplit) {
+                    if constexpr (BLOCK_N == 64) {
+                        if (p.blockdiag) {
 #pragma unroll
-                        for (int j = 0; j < 16; ++j) {
-                            raw[j] = __float_as_uint(__uint_as_float(raw[j]) + __uint_as_float(raw[16 + j]));
-                            raw[16 + j] = __float_as_uint(__uint_as_float(y[j]) + __uint_as_float(y[16 + j]));
+                            for (int k = 0; k < 4; ++k)
+#pragma unroll
+                                for (int q = 0; q < 8; ++q) d[8 * k + q] = d[16 * k + q] + d[16 * k + 8 + q];
+                            return;
                         }
-                        return;
                     }
-                    tmem_ld32(tb + (uint32_t)col0, raw); tmem_ld32(tb + (uint32_t)(BLOCK_N + col0), y);
-                } else {
-                    tmem_ld16(tb + (uint32_t)col0, raw); tmem_ld16(tb + (uint32_t)(BLOCK_N + col0), y);
-                }
-                tmem_wait_ld();
 #pragma unroll
-                for (int j = 0; j < CHUNK; ++j) raw[j] = __float_as_uint(__uint_as_float(raw[j]) + __uint_as_float(y[j]));
-            } else {
-                if constexpr (CHUNK == 32) tmem_ld32(tb + (uint32_t)col0, raw); else tmem_ld16(tb + (uint32_t)col0, raw);
-                tmem_wait_ld();
+                    for (int i = 0; i < BLOCK_N / 2; ++i) d[i] += d[i + BLOCK_N / 2];
+                }
             }
         };
+        // logical accumulator columns [c0, c0 + SW) of the whole tile -> scratch (both warpgroups), readable after the barrier
+        auto to_scratch = [&](int c0) {
+            epi_bar(3);
+            frag_to_scratch<BLOCK_N / 2, SW>(d, scr, 64 * wg, c0);
+            epi_bar(3);
+        };
+        // N logical columns [col0, col0 + N) of this thread's row, from the scratch chunk that holds them -> raw (fp32 bits)
+        auto ld_acc = [&](int col0, uint32_t* raw) {
+            scratch_row<SW, (BLOCK_N >= 32 ? 32 : 16)>(scr, row, col0 % SW, raw);
+        };
+        // Residual prefetch (TMA-store epilogue, split/bf16 residual): the 2 x 4 x 16 B of this thread's row for the NEXT 64-channel
+        // chunk are requested one chunk ahead, so their DRAM latency hides behind the current chunk (and the wait for the MMAs)
+        // instead of stalling every 8-channel group.
         uint4 rn_h[4], rn_l[4];
-        // compiled only into the instantiations that are dispatched with a residual (<*,2,3> and the halo <64,2,2>): the extra
-        // single-thread TMA issue path costs the others ~800 R2UR moves and 5-40 % of their speed (measured A/B on one box)
-        constexpr bool RES_TMA_OK = (STG == 3) || (STG == 2 && BLOCK_N == 64 && STAGES == 2);
+        // compiled only into the instantiations with at least two staging buffers (the ones dispatched with a residual)
+        constexpr bool RES_TMA_OK = (STG >= 2);
         const bool res_tma = RES_TMA_OK && p.res_tma && !(p.dbg & 8);
         constexpr bool RES_PF = (STG == 1 && BLOCK_N == 64);      // the halo configuration: no room for 3 staging buffers
         const bool res_pf = RES_PF && p.tma_out && p.res_split && !(p.dbg & 8);
@@ -337,7 +315,7 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             mbar_expect_tx(bar_res + 8 * buf_, (uint32_t)stg_bytes);
             tma_load_5d(smem_u32(stg) + buf_ * stg_bytes, &tmR, bar_res + 8 * buf_, (nt_ * BLOCK_N) % p.coutp + c64_ * 64, tw_ * p.TW, th_ * p.TH, img_, 0);
         };
-        if (res_tma && warp == 2 && lane == 0 && (int)blockIdx.x < total_tiles) res_tma_issue(blockIdx.x, 0, 0);
+        if (res_tma && warp == 4 && lane == 0 && (int)blockIdx.x < total_tiles) res_tma_issue(blockIdx.x, 0, 0);
         for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
             const int nt = tile % p.n_tiles, mt = tile / p.n_tiles;
             const int tw_i = mt % p.tiles_w; const int t2 = mt / p.tiles_w;
@@ -348,18 +326,18 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             const int q = n_glob / p.coutp, ch0 = n_glob % p.coutp;   // q = sub-position of a transposed conv (0 otherwise)
             const int ui = q / p.up, uj = q % p.up;
             const size_t pix = ((size_t)img * (p.Ho * p.up) + (size_t)(oh * p.up + ui)) * (size_t)(p.Wo * p.up) + (size_t)(ow * p.up + uj);
-            mbar_wait(bar_tfull + 8 * acc, acc_phase);
-            tc_fence_after();
+            mma_tile();
             if constexpr (STG > 0 && BLOCK_N >= 64) {
               if (p.tma_out) {
                 const uint32_t stg_base = smem_u32(stg);
 #pragma unroll 1
                 for (int c64 = 0; c64 < BLOCK_N / 64; ++c64) {
+                    to_scratch(c64 * 64);
                     const int b = stg_count % STG;
                     if (res_tma) {
                         // (A') the store that last used buffer (i+1) % STG has been read out -> request residual(i+1) into it, then wait
                         // for residual(i) in buffer b (STG == 3: a full chunk of lead; STG == 2: the lead is the chunk minus the store drain)
-                        if (warp == 2 && lane == 0) {
+                        if (warp == 4 && lane == 0) {
                             bulk_wait_read<(STG >= 2 ? STG - 2 : 0)>();
                             int ntile = tile, nc = c64 + 1;
                             if (nc == BLOCK_N / 64) { nc = 0; ntile = tile + (int)gridDim.x; }
@@ -368,7 +346,7 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                         mbar_wait(bar_res + 8 * b, (uint32_t)((stg_count / STG) & 1));
                     } else {
                         // (A) buffer b is free once at most STG-1 store groups are still reading shared memory
-                        if (warp == 2 && lane == 0) bulk_wait_read<STG - 1>();
+                        if (warp == 4 && lane == 0) bulk_wait_read<STG - 1>();
                         epi_bar(1);
                     }
                     // (B) this warp's 32 columns of the 64-column chunk -> registers -> epilogue -> swizzled smem.  Loads first (bias:
@@ -450,20 +428,20 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                     fence_async_smem();
                     epi_bar(2);
                     // (C) one thread drains the buffer with a TMA tensor store (out-of-range pixels are clipped by the unit)
-                    if (warp == 2 && lane == 0 && !(p.dbg & 1)) {
+                    if (warp == 4 && lane == 0 && !(p.dbg & 1)) {
                         tma_store_5d(&tmO, stg_base + b * stg_bytes, ch0 + c64 * 64, tw_i * p.TW, th_i * p.TH, img, 0);
                         bulk_commit();
                     }
                     ++stg_count;
                 }
-                tc_fence_before();
-                mbar_arrive(bar_tempty + 8 * acc);
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
                 continue;
               }
             }
 #pragma unroll 1
-            for (int cc = chalf; cc < BLOCK_N / CHUNK; cc += 2) {
+            for (int c0 = 0; c0 < BLOCK_N; c0 += SW) {
+                to_scratch(c0);
+                if (chalf >= SW / CHUNK) continue;
+                const int cc = c0 / CHUNK + chalf;
                 uint32_t raw[CHUNK];
                 ld_acc(cc * CHUNK, raw);
                 const int c_first = ch0 + cc * CHUNK;
@@ -539,18 +517,9 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                     }
                 }
             }
-            tc_fence_before();
-            mbar_arrive(bar_tempty + 8 * acc);          // 128 arrivals release this accumulator buffer
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
         }
-        if (STG > 0 && warp == 2 && lane == 0) bulk_wait_all();     // all output tiles have left shared memory
+        if (STG > 0 && warp == 4 && lane == 0) bulk_wait_all();     // all output tiles have left shared memory
         (void)stg_count;
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
     }
 }
 
@@ -568,11 +537,12 @@ const TcEnv& tc_env() { static const TcEnv e; return e; }
 template <int BLOCK_N, int STAGES, int STG, bool GELU = false>
 int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, const CUtensorMap& tmR, const TcP& p_in, cudaStream_t st) {
     TcP p = p_in;
-    p.res_tma = ((STG == 3 || (STG == 2 && BLOCK_N == 64 && STAGES == 2)) && p.tma_out && p.res_split && p_in.res_tma) ? 1 : 0;
+    p.res_tma = (STG >= 2 && p.tma_out && p.res_split && p_in.res_tma) ? 1 : 0;
     const size_t b_tile = p.bdiag ? (size_t)(BLOCK_N / 16) * 512 : (size_t)BLOCK_N * BLOCK_K * 2;
     size_t stage_bytes = (size_t)p.planes * A_TILE_BYTES + (size_t)p.wplanes * b_tile;
     if (p.halo) stage_bytes = (((size_t)p.planes * (p.TW + 2) * 128 + 1023) & ~(size_t)1023) + (size_t)p.wplanes * 3 * b_tile;
-    size_t smem = (size_t)STAGES * stage_bytes + (size_t)STG * p.planes * A_TILE_BYTES + 256;
+    const size_t scratch = (size_t)BLOCK_M * (BLOCK_N < 64 ? BLOCK_N : 64) * 4;
+    size_t smem = (size_t)STAGES * stage_bytes + (size_t)STG * p.planes * A_TILE_BYTES + scratch + 256;
     if (smem > 227 * 1024) return HEAL_ERR_UNSUPPORTED;
     static size_t attr_set[HEAL_MAX_DEVICES] = {};
     if (!heal_ensure_dyn_smem(k_conv2d_tc<BLOCK_N, STAGES, STG, GELU>, 227 * 1024, attr_set)) return HEAL_ERR_LAUNCH;
@@ -768,22 +738,24 @@ extern "C" int heal_conv2d_tc(const void* in_split, size_t in_plane_stride, int 
     if (relu == 2) {        // GELU: 1x1 / 3x3 convs with >= 128 output channels and no residual (ConvNeXt pwconv1: dim -> 4 dim)
         if (block_n != 128 || res_split || res_f32) return HEAL_ERR_UNSUPPORTED;
         if (!p.tma_out) return launch_tc<128, 3, 0, true>(tmA, tmB, tmO, tmR, p, st);
-        return kblocks <= 4 ? launch_tc<128, 2, 2, true>(tmA, tmB, tmO, tmR, p, st) : launch_tc<128, 3, 1, true>(tmA, tmB, tmO, tmR, p, st);
+        return kblocks <= 4 ? launch_tc<128, 2, 2, true>(tmA, tmB, tmO, tmR, p, st) : launch_tc<128, 2, 1, true>(tmA, tmB, tmO, tmR, p, st);
     }
+    // Configurations (stages, staging buffers) are sized to the 227 KiB of shared memory per block together with the
+    // 32 KiB fp32 accumulator scratch (split operands; planes == 1 needs less).
     switch (block_n) {
         case 16: return launch_tc<16, 4, 0>(tmA, tmB, tmO, tmR, p, st);
         case 32: return launch_tc<32, 4, 0>(tmA, tmB, tmO, tmR, p, st);
         case 64:
-            if (p.halo && res_tma_ok && !p.bdiag) return launch_tc<64, 2, 2>(tmA, tmB, tmO, tmR, p, st);   // 81 KiB stages + 2 x 32 KiB: all of shared memory
-            if (p.halo && p.bdiag && p.tma_out) return launch_tc<64, 4, 1>(tmA, tmB, tmO, tmR, p, st);     // 45 KiB stages
+            // halo: 81 KiB stages; a split residual is register-prefetched by the <64,2,1> epilogue
+            if (p.halo && p.bdiag && p.tma_out) return launch_tc<64, 3, 1>(tmA, tmB, tmO, tmR, p, st);     // 45 KiB stages
             if (p.halo) return p.tma_out ? launch_tc<64, 2, 1>(tmA, tmB, tmO, tmR, p, st) : launch_tc<64, 2, 0>(tmA, tmB, tmO, tmR, p, st);
-            if (p.bdiag && p.tma_out && !res_tma_ok) return launch_tc<64, 4, 2>(tmA, tmB, tmO, tmR, p, st);   // 36 KiB stages
+            if (p.bdiag && p.tma_out && !res_tma_ok) return launch_tc<64, 3, 2>(tmA, tmB, tmO, tmR, p, st);   // 36 KiB stages
             if (res_tma_ok) return launch_tc<64, 2, 3>(tmA, tmB, tmO, tmR, p, st);
-            return p.tma_out ? launch_tc<64, 3, 2>(tmA, tmB, tmO, tmR, p, st) : launch_tc<64, 4, 0>(tmA, tmB, tmO, tmR, p, st);
+            return p.tma_out ? launch_tc<64, 2, 2>(tmA, tmB, tmO, tmR, p, st) : launch_tc<64, 4, 0>(tmA, tmB, tmO, tmR, p, st);
         default:
             if (!p.tma_out) return launch_tc<128, 3, 0>(tmA, tmB, tmO, tmR, p, st);
-            if (res_tma_ok) return launch_tc<128, 2, 3>(tmA, tmB, tmO, tmR, p, st);
-            // HEAL_TC_DEEP=1 (experiment): 3 stages + 1 staging buffer also for the short-K layers
-            return (kblocks <= 4 && env.deep != 1) ? launch_tc<128, 2, 2>(tmA, tmB, tmO, tmR, p, st) : launch_tc<128, 3, 1>(tmA, tmB, tmO, tmR, p, st);
+            if (res_tma_ok) return launch_tc<128, 2, 2>(tmA, tmB, tmO, tmR, p, st);
+            // HEAL_TC_DEEP=1 (experiment): one staging buffer also for the short-K layers
+            return (kblocks <= 4 && env.deep != 1) ? launch_tc<128, 2, 2>(tmA, tmB, tmO, tmR, p, st) : launch_tc<128, 2, 1>(tmA, tmB, tmO, tmR, p, st);
     }
 }

@@ -1,10 +1,10 @@
 // Grouped 3x3 convolution (stride 1, pad 1; the ResNeXt bottleneck conv2, resblock.py:102-122 with groups = 32) as a ROW RING
-// on tcgen05: every input row is fetched from L2 ONCE and the weights ONCE per CTA.
+// on the Hopper tensor cores (wgmma): every input row is fetched from L2 ONCE and the weights ONCE per CTA.
 //
-// Why (ncu, profiles/ncu_r2/c2_conv_head_raw.csv): the tile-per-CTA kernel (k_conv2d_tc<64,4,1>, halo mode) pulls 700 MB through
-// the L2->SM crossbar for a 168 MB input at the 256x256 level -- each 130-pixel input row three times (once per kernel row) and
-// the 36 KB of packed weights once per 128-pixel tile -- with only four 45 KB stages in flight, and ends up bound by that
-// latency (117 us; 72 us with the MMAs removed) instead of by the 42 us of MMA issue.
+// Why: the tile-per-CTA kernel (k_conv2d_tc<64,*,1>, halo mode) pulls each 130-pixel input row through the L2->SM crossbar
+// three times (once per kernel row) and the 36 KB of packed weights once per 128-pixel tile -- about 4x the input size at the
+// 256x256 level -- with only a few 45 KB stages in flight, and was bound by that latency rather than by MMA issue (profiled on
+// the B200 build; not re-profiled on the H100).
 //
 // Here a CTA owns a vertical strip: (image, 128-pixel column tile, 64-channel block) x a range of rows.  Shared memory holds
 //   * a ring of R input rows, each [plane][130 pixels][64 channels] bf16 as written by one 5-D TMA box (128B swizzle; rows
@@ -14,9 +14,10 @@
 // Output row h needs ring rows h-1, h, h+1: the three horizontal taps are row-shifted descriptors of the same ring row (the
 // swizzle is a function of the absolute shared-memory address), so one new row per output row is all that is loaded.
 // Precision and MMA forms are those of conv2d_tc.cu: a_hi x [b_hi | b_lo] as one N = 32 MMA plus a_lo x b_hi as an N = 16 MMA
-// per 16-channel sub-block and tap, fp32 accumulation in TMEM, two accumulator buffers (the epilogue of row h overlaps the
-// MMAs of row h+1).  Roles: warp 0 TMA producer, warp 1 MMA issuer, warps 2..9 epilogue (bias, ReLU, hi/lo split, swizzled
-// staging, one TMA tensor store per row).
+// per 16-channel sub-block and tap, fp32 accumulation in registers.  Roles: warpgroup 0 = TMA producer (warp 0); warpgroups 1
+// and 2 = the M = 64 wgmma of one half of the row tile each, then the epilogue of the whole row (accumulators transposed
+// through an fp32 scratch that shares the bytes of the output staging tile, bias, ReLU, hi/lo split, swizzled staging, one
+// TMA tensor store per row).
 #include <cuda.h>
 #include "common.cuh"
 #include "tc_prims.cuh"
@@ -24,16 +25,18 @@
 
 namespace {
 
-constexpr int RG_THREADS = 320;
+constexpr int RG_THREADS = 384;
 constexpr int RG_TW = 128;                          // output pixels per row tile = MMA M
 constexpr int RG_ROW_PLANE = (RG_TW + 2) * 128;     // one plane of one ring row: 130 pixels x 64 channels bf16
 constexpr int RG_STG_PLANE = RG_TW * 128;           // one plane of the output staging tile
 constexpr int RG_MAX_SLOTS = 8;
-constexpr int RG_TMEM_COLS = 256;                   // 2 accumulators x 128 columns
+constexpr int RG_SCRATCH = RG_TW * 64 * 4;          // fp32 accumulator scratch [128 rows][64 channels]
 constexpr int RG_SMEM_LIMIT = 227 * 1024;
 
 __host__ __device__ inline int rg_slot_bytes(int planes) { return (planes * RG_ROW_PLANE + 1023) & ~1023; }
 __host__ __device__ inline int rg_wrow_bytes(int wplanes) { return 3 * 4 * wplanes * 512; }   // one kernel row: [3 taps][4 sub-blocks][plane][16][32 B]
+// output staging tile, also the accumulator scratch
+__host__ __device__ inline int rg_stg_bytes(int planes) { return planes * RG_STG_PLANE > RG_SCRATCH ? planes * RG_STG_PLANE : RG_SCRATCH; }
 
 __global__ void __launch_bounds__(RG_THREADS, 1)
 k_gconv3x3_ring(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -56,102 +59,56 @@ k_gconv3x3_ring(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     if (smem_u32(smem) & 1023u) __trap();
     const int slot_bytes = rg_slot_bytes(p.planes);
     const int wrow_bytes = rg_wrow_bytes(p.wplanes);
-    const int stg_bytes = p.planes * RG_STG_PLANE;
+    const int stg_bytes = rg_stg_bytes(p.planes);
     const uint32_t ring = smem_u32(smem);
     const uint32_t wbase = ring + (uint32_t)(slots * slot_bytes);
     const uint32_t stg = wbase + (uint32_t)(3 * wrow_bytes);
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)slots * slot_bytes + 3 * wrow_bytes + stg_bytes);
-    // bars: full[8], empty[8], wfull, tfull[2], tempty[2]
+    // bars: full[8], empty[8], wfull
     const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + RG_MAX_SLOTS), bar_w = smem_u32(bars + 2 * RG_MAX_SLOTS);
-    const uint32_t bar_tfull = smem_u32(bars + 2 * RG_MAX_SLOTS + 1), bar_tempty = smem_u32(bars + 2 * RG_MAX_SLOTS + 3);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * RG_MAX_SLOTS + 6);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
-        for (int s = 0; s < RG_MAX_SLOTS; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 1); }
+        for (int s = 0; s < RG_MAX_SLOTS; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 8); }   // 8 consumer warps
         mbar_init(bar_w, 1);
-        for (int a = 0; a < 2; ++a) { mbar_init(bar_tfull + 8 * a, 1); mbar_init(bar_tempty + 8 * a, 256); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(RG_TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     const bool split = (p.planes == 2), wsplit = (p.wplanes == 2);
-    // programmatic dependent launch: barrier init / TMEM allocation above overlapped the previous kernel's tail; nothing it
-    // produced has been touched yet
+    // programmatic dependent launch: the barrier init above overlapped the previous kernel's tail; nothing it produced has
+    // been touched yet
     if (p.pdl) {
         asm volatile("griddepcontrol.wait;" ::: "memory");
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     }
 
-    if (warp == 0) {
-        // ============================== TMA producer ==============================
-        if (elect_one()) {
-            mbar_expect_tx(bar_w, (uint32_t)(3 * wrow_bytes));
-            for (int r = 0; r < 3; ++r) tma_load_5d(wbase + r * wrow_bytes, &tmB, bar_w, 0, 0, 0, cb * 4, r * 3);
-        }
-        __syncwarp();
-        const int n_in = rows + 2;                       // input rows h_begin-1 .. h_begin+rows
-        for (int j = 0; j < n_in; ++j) {
-            const int slot = j % slots, use = j / slots;
-            mbar_wait(bar_empty + 8 * slot, (uint32_t)((use & 1) ^ 1));
+    if (warp < 4) {
+        regs_dec<40>();
+        // ============================== TMA producer (warp 0) =====================
+        if (warp == 0) {
             if (elect_one()) {
-                mbar_expect_tx(bar_full + 8 * slot, (uint32_t)(p.planes * RG_ROW_PLANE));
-                tma_load_5d(ring + slot * slot_bytes, &tmA, bar_full + 8 * slot, cb * 64, w0 - 1, h_begin - 1 + j, img, 0);
+                mbar_expect_tx(bar_w, (uint32_t)(3 * wrow_bytes));
+                for (int r = 0; r < 3; ++r) tma_load_5d(wbase + r * wrow_bytes, &tmB, bar_w, 0, 0, 0, cb * 4, r * 3);
             }
             __syncwarp();
-        }
-    } else if (warp == 1) {
-        // ============================== MMA issuer ================================
-        const uint32_t idesc16 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(16 >> 3) << 17) | ((uint32_t)(RG_TW >> 4) << 24);
-        const uint32_t idesc32 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(32 >> 3) << 17) | ((uint32_t)(RG_TW >> 4) << 24);
-        const int sub_cols = wsplit ? 32 : 16;           // accumulator columns per 16-channel sub-block: [main16 | aux16]
-        const uint32_t tap_bytes = (uint32_t)(4 * p.wplanes * 512), sub_bytes = (uint32_t)(p.wplanes * 512);
-        mbar_wait(bar_w, 0);
-        int waited = 0, acc = 0; uint32_t acc_phase = 0;
-        for (int t = 0; t < rows; ++t) {
-            mbar_wait(bar_tempty + 8 * acc, acc_phase ^ 1);
-            while (waited < t + 3) { mbar_wait(bar_full + 8 * (waited % slots), (uint32_t)((waited / slots) & 1)); ++waited; }
-            tc_fence_after();
-            const uint32_t tmem_d = tmem_base + (uint32_t)(acc * 128);
-            if (elect_one()) {
-                for (int r = 0; r < 3; ++r) {
-                    const uint32_t sa = ring + (uint32_t)(((t + r) % slots) * slot_bytes);
-#pragma unroll
-                    for (int s = 0; s < 3; ++s) {
-                        const uint32_t ah = sa + s * 128, al = ah + RG_ROW_PLANE;      // tap s = rows [s, s+128) of the 130-row tile
-                        const uint32_t bs = wbase + r * wrow_bytes + s * tap_bytes;
-                        const uint32_t f0 = (r == 0 && s == 0) ? 0u : 1u;
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            const uint64_t a_hi = umma_desc_sw128(ah + k * 32);
-                            const uint64_t bd = umma_desc_sw32(bs + k * sub_bytes);
-                            const uint32_t td = tmem_d + (uint32_t)(k * sub_cols);
-                            if (wsplit) {
-                                umma_bf16(td, a_hi, bd, idesc32, f0);                                    // [a_hi*b_hi | a_hi*b_lo]
-                                if (split) umma_bf16(td, umma_desc_sw128(al + k * 32), bd, idesc16, 1u); // += a_lo*b_hi
-                            } else {
-                                umma_bf16(td, a_hi, bd, idesc16, f0);
-                            }
-                        }
-                    }
+            const int n_in = rows + 2;                       // input rows h_begin-1 .. h_begin+rows
+            for (int j = 0; j < n_in; ++j) {
+                const int slot = j % slots, use = j / slots;
+                mbar_wait(bar_empty + 8 * slot, (uint32_t)((use & 1) ^ 1));
+                if (elect_one()) {
+                    mbar_expect_tx(bar_full + 8 * slot, (uint32_t)(p.planes * RG_ROW_PLANE));
+                    tma_load_5d(ring + slot * slot_bytes, &tmA, bar_full + 8 * slot, cb * 64, w0 - 1, h_begin - 1 + j, img, 0);
                 }
-                umma_commit(bar_empty + 8 * (t % slots));    // input row h-1 is not needed by any later output row
-                umma_commit(bar_tfull + 8 * acc);
+                __syncwarp();
             }
-            __syncwarp();
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
         }
     } else {
-        // ============================== epilogue (warps 2..9) =====================
-        const int quarter = warp & 3;                   // TMEM lane quarter this warp may access
-        const int chalf = (warp - 2) >> 2;              // which 32 of the 64 channels this warp drains
-        const int row = quarter * 32 + lane;            // pixel within the row tile
+        // ============================== consumers: wgmma + epilogue ===============
+        regs_inc<232>();
+        const int wg = (warp >> 2) - 1;                 // MMAs: pixels [64 wg, 64 wg + 64) of the row tile
+        const int quarter = warp & 3;
+        const int chalf = (warp - 4) >> 2;              // epilogue: which 32 of the 64 channels this warp drains
+        const int row = quarter * 32 + lane;            // epilogue: pixel within the row tile
         const uint32_t srow = stg + (uint32_t)(row * 128);
         float bv[32];
 #pragma unroll
@@ -159,28 +116,52 @@ k_gconv3x3_ring(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             float4 b4 = p.bias ? __ldg(reinterpret_cast<const float4*>(p.bias + cb * 64 + chalf * 32) + g) : make_float4(0.f, 0.f, 0.f, 0.f);
             bv[4 * g] = b4.x; bv[4 * g + 1] = b4.y; bv[4 * g + 2] = b4.z; bv[4 * g + 3] = b4.w;
         }
-        int acc = 0; uint32_t acc_phase = 0;
-        for (int t = 0; t < rows; ++t) {
-            mbar_wait(bar_tfull + 8 * acc, acc_phase);
-            tc_fence_after();
-            const uint32_t tb = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * 128);
-            uint32_t raw[32];
-            if (wsplit) {
-                uint32_t y[32];
-                tmem_ld32(tb + (uint32_t)(chalf * 64), raw); tmem_ld32(tb + (uint32_t)(chalf * 64 + 32), y);
-                tmem_wait_ld();
+        const uint32_t tap_bytes = (uint32_t)(4 * p.wplanes * 512), sub_bytes = (uint32_t)(p.wplanes * 512);
+        float d[64];
 #pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    raw[j] = __float_as_uint(__uint_as_float(raw[j]) + __uint_as_float(raw[16 + j]));
-                    raw[16 + j] = __float_as_uint(__uint_as_float(y[j]) + __uint_as_float(y[16 + j]));
+        for (int i = 0; i < 64; ++i) d[i] = 0.f;
+        mbar_wait(bar_w, 0);
+        int waited = 0;
+        for (int t = 0; t < rows; ++t) {
+            while (waited < t + 3) { mbar_wait(bar_full + 8 * (waited % slots), (uint32_t)((waited / slots) & 1)); ++waited; }
+            wgmma_fence();
+            for (int r = 0; r < 3; ++r) {
+                const uint32_t sa = ring + (uint32_t)(((t + r) % slots) * slot_bytes) + (uint32_t)(wg * 64 * 128);
+#pragma unroll
+                for (int s = 0; s < 3; ++s) {
+                    const uint32_t ah = sa + s * 128, al = ah + RG_ROW_PLANE;      // tap s = rows [s, s+128) of the 130-row tile
+                    const uint32_t bs = wbase + r * wrow_bytes + s * tap_bytes;
+                    const uint32_t f0 = (r == 0 && s == 0) ? 0u : 1u;
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                        const uint64_t a_hi = gmma_desc_sw128(ah + k * 32);
+                        const uint64_t bd = gmma_desc_sw32(bs + k * sub_bytes);
+                        if (wsplit) {
+                            wgmma_bf16<32>(d + 16 * k, a_hi, bd, f0);                                    // [a_hi*b_hi | a_hi*b_lo]
+                            if (split) wgmma_bf16<16>(d + 16 * k, gmma_desc_sw128(al + k * 32), bd, 1u); // += a_lo*b_hi
+                        } else {
+                            wgmma_bf16<16>(d + 8 * k, a_hi, bd, f0);
+                        }
+                    }
                 }
-            } else {
-                tmem_ld32(tb + (uint32_t)(chalf * 32), raw);
-                tmem_wait_ld();
             }
-            // accumulator consumed: hand the buffer back before the stores
-            tc_fence_before();
-            mbar_arrive(bar_tempty + 8 * acc);
+            wgmma_commit();
+            wgmma_wait<0>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(bar_empty + 8 * (t % slots));    // input row h-1 is not needed by any later output row
+            if (wsplit) {          // [main16 | aux16] per sub-block -> 64 logical columns
+#pragma unroll
+                for (int k = 0; k < 4; ++k)
+#pragma unroll
+                    for (int q = 0; q < 8; ++q) d[8 * k + q] = d[16 * k + q] + d[16 * k + 8 + q];
+            }
+            // the previous row's TMA store has finished reading the staging tile, which now takes the accumulators
+            if (warp == 4 && lane == 0) bulk_wait_read<0>();
+            epi_bar(1);
+            frag_to_scratch<32, 64>(d, stg, 64 * wg, 0);
+            epi_bar(1);
+            uint32_t raw[32];
+            scratch_row<64, 32>(stg, row, chalf * 32, raw);
             uint32_t hw[4][4], lw[4][4];
 #pragma unroll
             for (int g8 = 0; g8 < 4; ++g8) {
@@ -194,9 +175,7 @@ k_gconv3x3_ring(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 #pragma unroll
                 for (int j = 0; j < 4; ++j) { hw[g8][j] = pack_bf16(v[2 * j], v[2 * j + 1]); lw[g8][j] = pack_bf16(lo[2 * j], lo[2 * j + 1]); }
             }
-            // the previous row's TMA store has finished reading the staging tile
-            if (warp == 2 && lane == 0) bulk_wait_read<0>();
-            epi_bar(1);
+            epi_bar(1);            // every scratch read is done before the staging tile is overwritten
 #pragma unroll
             for (int g8 = 0; g8 < 4; ++g8) {
                 const uint32_t chunk16 = (uint32_t)(((chalf * 4 + g8) ^ (row & 7)) * 16);      // 128B swizzle
@@ -206,19 +185,12 @@ k_gconv3x3_ring(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             }
             fence_async_smem();
             epi_bar(2);
-            if (warp == 2 && lane == 0) {
+            if (warp == 4 && lane == 0) {
                 tma_store_5d(&tmO, stg, cb * 64, w0, h_begin + t, img, 0);
                 bulk_commit();
             }
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
         }
-        if (warp == 2 && lane == 0) bulk_wait_all();     // the last tile has left shared memory
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(RG_TMEM_COLS) : "memory");
+        if (warp == 4 && lane == 0) bulk_wait_all();     // the last tile has left shared memory
     }
 }
 
@@ -226,7 +198,7 @@ k_gconv3x3_ring(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 
 int heal_conv3x3_ring_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, RingP p, cudaStream_t st) {
     if ((p.W % RG_TW) || (p.C % 64) || p.N < 1 || p.H < 1) return HEAL_ERR_UNSUPPORTED;
-    const int slot_bytes = rg_slot_bytes(p.planes), w_bytes = 3 * rg_wrow_bytes(p.wplanes), stg_bytes = p.planes * RG_STG_PLANE;
+    const int slot_bytes = rg_slot_bytes(p.planes), w_bytes = 3 * rg_wrow_bytes(p.wplanes), stg_bytes = rg_stg_bytes(p.planes);
     int slots = (RG_SMEM_LIMIT - w_bytes - stg_bytes - 512) / slot_bytes;
     if (slots > RG_MAX_SLOTS) slots = RG_MAX_SLOTS;
     if (slots < 4) return HEAL_ERR_UNSUPPORTED;

@@ -1,7 +1,7 @@
 // ConvNeXt aligner front half: depthwise k x k convolution + bias + LayerNorm over the channels of every pixel, one kernel.
 // Reference: opencood/models/sub_modules/feature_alignnet_modules.py:299-345 (ConvNeXtBlock: dwconv -> permute -> LayerNorm(eps 1e-6,
 // channels_last, :12-25) -> Linear -> GELU -> Linear -> gamma -> + input).  The two Linear layers are 1x1 convolutions and run on
-// the tcgen05 conv engine (csrc/conv2d_tc.cu, GELU / residual in its epilogue); this kernel produces their input.
+// the wgmma conv engine (csrc/conv2d_tc.cu, GELU / residual in its epilogue); this kernel produces their input.
 // HBM-bound: reads the map once (the 7x7 neighbourhood of a pixel is shared through L1/L2 by the warps of a block, which cover
 // 8 x 4 neighbouring pixels), writes it once.  One warp per pixel, lane = channel pair (C = 64) -> every tap is one coalesced
 // 256 B (fp32) row read; mean / variance by warp shuffles, exactly LayerNorm's biased variance.

@@ -319,8 +319,8 @@ k_att_fuse(AttP p) {
 }
 
 // Split-bf16 features, 8 channels per lane (16-byte loads per plane and tap), C <= 256: half the load instructions of the
-// generic kernel and 128-thread blocks (4 pixels) for more resident blocks per SM -- the generic version ran at 23 % achieved
-// occupancy with 8-byte loads and was latency-bound at 0.6 TB/s (ncu, profiles/ncu_full_r2_summary.json).
+// generic kernel and 128-thread blocks (4 pixels) for more resident blocks per SM -- the generic version, with 8-byte loads and
+// larger blocks, was latency-bound under a profiler on the B200 build.
 template <int NA>
 __global__ void __launch_bounds__(128)
 k_att_fuse_split8(AttP p) {

@@ -213,7 +213,7 @@ k_iou_mask(const double* __restrict__ poly, const int* __restrict__ counters, in
 // One block: all threads stage the suppression matrix (top x words x 8 B <= 128 KiB for top = 1000) and the in-range flags in shared
 // memory, then warp 0 does the greedy scan from there and lists the survivors that are also in range; k_emit copies them in
 // parallel.  (Reading the mask row and the corners of every kept box straight from global memory inside the scan costs two
-// dependent ~0.5 us loads per box: 0.5 ms per frame.)
+// dependent global-memory loads per box on the serial path.)
 __global__ void __launch_bounds__(1024)
 k_nms_finish(const unsigned long long* __restrict__ mask, const unsigned char* __restrict__ inrange, const int* __restrict__ counters,
              int top, int words, int* __restrict__ keep_idx, int* __restrict__ count_out) {

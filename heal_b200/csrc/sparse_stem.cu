@@ -77,8 +77,8 @@ k_sparse_stem(StemP p) {
 }
 
 // ---- tensor-core variant (split-bf16, fp32-equivalent) ------------------------------------------------------------------------
-// The SIMT kernel above streams a 16 KB tap matrix from L1 for every occupied (pixel, tap) pair and is bound by that (190 us,
-// 110 M warp instructions at 5 x 512^2).  Here a warp owns 16 consecutive output pixels of a row (one m16 row block of
+// The SIMT kernel above streams a 16 KB tap matrix from L1 for every occupied (pixel, tap) pair and is bound by that
+// (110 M warp instructions at 5 x 512^2).  Here a warp owns 16 consecutive output pixels of a row (one m16 row block of
 // mma.sync.m16n8k16) and keeps both 16x64 fp32 outputs in registers; for each of the 9 taps that has at least one hit among the 16
 // pixels it gathers the hit pillars' features as the A fragments (zero rows elsewhere), splits them into bf16 hi/lo and issues
 // a_lo*b_hi + a_hi*b_lo + a_hi*b_hi against the tap's 64x64 weights, which all ten matrices (9 taps + the 1x1 downsample) keep

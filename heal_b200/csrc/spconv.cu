@@ -6,7 +6,7 @@
 //   SubMConv3d   : output sites = input sites;
 //   SparseConv3d : output sites = every site reached by at least one active input under the kernel,
 //                  out = floor((in + 2*pad - k) / stride) + 1 per axis.
-// B200 design: "output-stationary" rulebook. For each output row we store the input row feeding each of the K
+// Design: "output-stationary" rulebook. For each output row we store the input row feeding each of the K
 // kernel offsets (-1 if inactive), built with a GPU hash table; the convolution is then ONE gather-GEMM kernel per
 // layer with BatchNorm1d folded and ReLU fused, no atomics and no intermediate buffers, deterministic per row.
 // Output-site order of a strided conv = order of first generation by (input row, kernel offset), made

@@ -1,4 +1,4 @@
-// Sparse 3-D convolution gather-GEMM on the 5th-generation tensor cores (tcgen05.mma, accumulators in TMEM) for the
+// Sparse 3-D convolution gather-GEMM on the Hopper tensor cores (wgmma, fp32 accumulators in registers) for the
 // SECOND middle encoder (VoxelBackBone8x; reference layer list: opencood/models/sub_modules/sparse_backbone_3d.py:48-91,
 // post_act_block :11-30 = conv + BatchNorm1d(eps 1e-3) + ReLU; spconv semantics restated in oracle/sparse_conv.py).
 //
@@ -10,14 +10,15 @@
 // Features travel between layers as "split rows": (rows, 2*C) bf16 = [hi C | lo C], x ~= hi + lo (16 mantissa bits),
 // and a product is a_hi*b_hi + a_hi*b_lo + a_lo*b_hi with fp32 accumulation: fp32-equivalent (same scheme as conv2d_tc.cu).
 //
-// Roles (288 threads, persistent over tiles):
+// Roles (384 threads, persistent over tiles):
 //   warps 0..3  gather producers: the tile's rulebook rows go to shared memory once; per ACTIVE K-block (a K-block none of
 //               the tile's 128 rows hits is skipped altogether) every thread issues sixteen 16-byte cp.async copies (8 lanes
 //               per gathered row: full 128 B lines; src-size 0 zero-fills a miss) into the 128B-swizzled K-major A tile, and
 //               one lane TMA-loads the K-block's weights.  Copies stay in flight across K-blocks and tiles (cp.async groups,
 //               two behind), then fence.proxy.async + mbarrier arrive hand the stage to the tensor core.
-//   warp  4     MMA issuer: 4 K-steps x { a_hi x [b_hi | b_lo] (N' = 2 Cout), a_lo x b_hi } per stage, double-buffered TMEM.
-//   warps 5..8  epilogue: TMEM -> registers -> main + aux -> + BN shift -> ReLU -> split rows (or fp32 rows) to global.
+//   warps 4..11 two consumer warpgroups, rows [0, 64) and [64, 128) of the tile: 4 K-steps x { a_hi x [b_hi | b_lo] (N' = 2 Cout),
+//               a_lo x b_hi } per stage (Cout = 128: three N = 128 products), then the epilogue: main + aux -> fp32 scratch in
+//               shared memory (one row per thread) -> + BN shift -> ReLU -> split rows (or fp32 rows) to global.
 #include <cuda.h>
 #include "common.cuh"
 #include "tc_prims.cuh"
@@ -25,7 +26,7 @@
 
 namespace {
 
-constexpr int SPT_THREADS = 288;
+constexpr int SPT_THREADS = 384;
 constexpr int SPT_M = 128;
 constexpr int SPT_ATILE = SPT_M * 128;          // one plane of A: 128 rows x 128 B
 
@@ -52,8 +53,9 @@ k_spconv_tc(const __grid_constant__ CUtensorMap tmB, const SptP p) {
     constexpr int CPT = CIN / 8;                    // 16-byte chunks per gathered row and plane
     constexpr int B_BYTES = 2 * COUT * 128;         // [plane][COUT rows][128 B]
     constexpr int STAGE_BYTES = 2 * SPT_ATILE + B_BYTES;
-    constexpr int ACC_STRIDE = 2 * COUT;            // main | aux accumulator columns
-    constexpr int TMEM_COLS = (2 * ACC_STRIDE < 32) ? 32 : 2 * ACC_STRIDE;
+    constexpr bool NCAT = (COUT <= 64);             // a_hi x [b_hi | b_lo] as one N = 2 COUT product
+    constexpr int NACC = NCAT ? 2 * COUT : COUT;    // accumulator columns (main | aux)
+    constexpr int SW = COUT < 64 ? COUT : 64;       // accumulator columns per pass through the scratch
     constexpr int LA = (STAGES >= 4) ? 2 : 1;       // cp.async groups a producer keeps in flight behind the one it issues
     constexpr int KPAD = 28;                        // rulebook row pitch in shared memory (K <= 27)
 
@@ -62,29 +64,20 @@ k_spconv_tc(const __grid_constant__ CUtensorMap tmB, const SptP p) {
     asm volatile("" : "+l"(raw_addr));
     uint8_t* smem = reinterpret_cast<uint8_t*>(raw_addr);
     if (smem_u32(smem) & 1023u) __trap();
-    int* snbr = reinterpret_cast<int*>(smem + (size_t)STAGES * STAGE_BYTES);
+    const uint32_t scr = smem_u32(smem + (size_t)STAGES * STAGE_BYTES);   // fp32 scratch [128 rows][SW]
+    int* snbr = reinterpret_cast<int*>(smem + (size_t)STAGES * STAGE_BYTES + SPT_M * SW * 4);
     int* sflags = snbr + SPT_M * KPAD;                                  // [STAGES] bit0 = first K-block of its tile, bit1 = last
     unsigned* smask = reinterpret_cast<unsigned*>(sflags + STAGES);     // [2] active-K-block mask of the tile being set up
     uint64_t* bars = reinterpret_cast<uint64_t*>((reinterpret_cast<uintptr_t>(smask + 2) + 7) & ~(uintptr_t)7);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
     const uint32_t smem_base = smem_u32(smem);
     const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + STAGES);
-    const uint32_t bar_tfull = smem_u32(bars + 2 * STAGES), bar_tempty = smem_u32(bars + 2 * STAGES + 2);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(bar_full + 8 * s, 128 + 1); mbar_init(bar_empty + 8 * s, 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(bar_tfull + 8 * a, 1); mbar_init(bar_tempty + 8 * a, 128); }
+        for (int s = 0; s < STAGES; ++s) { mbar_init(bar_full + 8 * s, 128 + 1); mbar_init(bar_empty + 8 * s, 8); }   // 8 consumer warps
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 4) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     const int Md = p.m_dev ? min(p.M, p.m_dev[0]) : p.M;
     const int ntiles = (Md + SPT_M - 1) / SPT_M;
@@ -98,7 +91,7 @@ k_spconv_tc(const __grid_constant__ CUtensorMap tmB, const SptP p) {
         for (int i = 0; i <= LA; ++i) pend[i] = 0;
         // The tile's rulebook rows (128 x K ints, contiguous) are prefetched into REGISTERS one tile ahead: the loads fly under the
         // current tile's gathers, so a tile starts without an exposed global-memory round trip (the first version re-read them at
-        // every tile start: ~2 us of bubble per tile, profiles/ncu_full_r2_summary.json: long_scoreboard-bound at 14 % occupancy)
+        // every tile start and stalled on that round trip)
         int nxt[27];
         auto fetch = [&](int tile_) {
             const long long base = (long long)tile_ * SPT_M * p.K;
@@ -176,104 +169,105 @@ k_spconv_tc(const __grid_constant__ CUtensorMap tmB, const SptP p) {
         cp_async_wait<0>();
         fence_async_smem();
         for (int i = 0; i < npend; ++i) mbar_arrive(bar_full + 8 * pend[i]);
-    } else if (warp == 4) {
-        // ================================ MMA issuer ================================
-        const uint32_t idesc_cat = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)((2 * COUT) >> 3) << 17) | ((uint32_t)(SPT_M >> 4) << 24);
-        const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(COUT >> 3) << 17) | ((uint32_t)(SPT_M >> 4) << 24);
+    } else {
+        // ================================ consumers: wgmma + epilogue ================================
+        const int wg = (warp >> 2) - 1;                // MMAs: tile rows [64 wg, 64 wg + 64)
+        const int quarter = warp & 3;
+        const int chalf = (warp - 4) >> 2;             // epilogue: which half of each scratch chunk this warp drains
+        const int row = quarter * 32 + lane;
+        constexpr int CH = (COUT >= 32) ? 32 : 16;
+        float d[NACC / 2];
+#pragma unroll
+        for (int i = 0; i < NACC / 2; ++i) d[i] = 0.f;
         int stage = 0; uint32_t phase = 0;
-        int acc = 0; uint32_t acc_phase = 0;
         for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-            mbar_wait(bar_tempty + 8 * acc, acc_phase ^ 1);
-            tc_fence_after();
-            const uint32_t tmem_d = tmem_base + (uint32_t)(acc * ACC_STRIDE);
+            int prev = -1;
             while (true) {
                 mbar_wait(bar_full + 8 * stage, phase);
-                tc_fence_after();
                 const int fl = sflags[stage];
-                const uint32_t sa = smem_base + stage * STAGE_BYTES;
-                const uint32_t sb = sa + 2 * SPT_ATILE;
-                if (elect_one()) {
+                const uint32_t sa = smem_base + stage * STAGE_BYTES + (uint32_t)(wg * 64 * 128);
+                const uint32_t sb = smem_base + stage * STAGE_BYTES + 2 * SPT_ATILE;
+                wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const uint64_t a_hi = umma_desc_sw128(sa + k * 32), a_lo = umma_desc_sw128(sa + SPT_ATILE + k * 32);
-                        const uint64_t b = umma_desc_sw128(sb + k * 32);
-                        umma_bf16(tmem_d, a_hi, b, idesc_cat, ((fl & 1) && k == 0) ? 0u : 1u);   // [a_hi*b_hi | a_hi*b_lo]
-                        umma_bf16(tmem_d, a_lo, b, idesc, 1u);                                   // += a_lo*b_hi
+                for (int k = 0; k < 4; ++k) {
+                    const uint64_t a_hi = gmma_desc_sw128(sa + k * 32), a_lo = gmma_desc_sw128(sa + SPT_ATILE + k * 32);
+                    const uint64_t b = gmma_desc_sw128(sb + k * 32);
+                    const uint32_t first = ((fl & 1) && k == 0) ? 0u : 1u;
+                    if constexpr (NCAT) {
+                        wgmma_bf16<2 * COUT>(d, a_hi, b, first);                  // [a_hi*b_hi | a_hi*b_lo]
+                        wgmma_bf16<COUT>(d, a_lo, b, 1u);                         // += a_lo*b_hi
+                    } else {
+                        wgmma_bf16<COUT>(d, a_hi, gmma_desc_sw128(sb + COUT * 128 + k * 32), first);   // a_hi*b_lo
+                        wgmma_bf16<COUT>(d, a_lo, b, 1u);
+                        wgmma_bf16<COUT>(d, a_hi, b, 1u);
                     }
-                    umma_commit(bar_empty + 8 * stage);
                 }
-                __syncwarp();
+                wgmma_commit();
+                // The producers hand a stage over LA stages late (cp.async groups in flight), so keeping one stage of MMAs in
+                // flight here as well needs STAGES > LA + 1: otherwise both sides wait for each other.
+                if constexpr (STAGES > LA + 1) {
+                    wgmma_wait<1>();                   // the previous stage's MMAs have retired: free it
+                    if (prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev);
+                    prev = stage;
+                } else {
+                    wgmma_wait<0>();
+                    if (lane == 0) mbar_arrive(bar_empty + 8 * stage);
+                }
                 if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 if (fl & 2) break;
             }
-            if (elect_one()) umma_commit(bar_tfull + 8 * acc);
-            __syncwarp();
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-        }
-    } else {
-        // ================================ epilogue ================================
-        const int quarter = warp & 3;                  // TMEM lane quarter this warp may access (warps 5,6,7,8 -> 1,2,3,0)
-        const int row = quarter * 32 + lane;
-        constexpr int CH = (COUT >= 32) ? 32 : 16;
-        int acc = 0; uint32_t acc_phase = 0;
-        for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+            wgmma_wait<0>();
+            if (prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev);
+            if constexpr (NCAT) {
+#pragma unroll
+                for (int i = 0; i < COUT / 2; ++i) d[i] += d[i + COUT / 2];
+            }
             const int grow = tile * SPT_M + row;
-            mbar_wait(bar_tfull + 8 * acc, acc_phase);
-            tc_fence_after();
-            const uint32_t tb = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * ACC_STRIDE);
 #pragma unroll 1
-            for (int c0 = 0; c0 < COUT; c0 += CH) {
-                uint32_t x[CH], y[CH];
-                if constexpr (CH == 32) { tmem_ld32(tb + (uint32_t)c0, x); tmem_ld32(tb + (uint32_t)(COUT + c0), y); }
-                else { tmem_ld16(tb + (uint32_t)c0, x); tmem_ld16(tb + (uint32_t)(COUT + c0), y); }
-                tmem_wait_ld();
-                if (grow < Md) {
+            for (int cs = 0; cs < COUT; cs += SW) {
+                epi_bar(1);
+                frag_to_scratch<COUT / 2, SW>(d, scr, 64 * wg, cs);
+                epi_bar(1);
+                if (chalf >= SW / CH || grow >= Md) continue;
+                const int c0 = cs + chalf * CH;
+                uint32_t x[CH];
+                scratch_row<SW, CH>(scr, row, chalf * CH, x);
 #pragma unroll
-                    for (int g8 = 0; g8 < CH / 8; ++g8) {
-                        float v[8];
+                for (int g8 = 0; g8 < CH / 8; ++g8) {
+                    float v[8];
 #pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            v[j] = __uint_as_float(x[g8 * 8 + j]) + __uint_as_float(y[g8 * 8 + j]) + (p.bias ? __ldg(p.bias + c0 + g8 * 8 + j) : 0.f);
-                            if (p.relu) v[j] = fmaxf(v[j], 0.f);
-                        }
-                        if (p.out_split) {
-                            uint32_t hw[4], lw[4];
+                    for (int j = 0; j < 8; ++j) {
+                        v[j] = __uint_as_float(x[g8 * 8 + j]) + (p.bias ? __ldg(p.bias + c0 + g8 * 8 + j) : 0.f);
+                        if (p.relu) v[j] = fmaxf(v[j], 0.f);
+                    }
+                    if (p.out_split) {
+                        uint32_t hw[4], lw[4];
 #pragma unroll
-                            for (int j = 0; j < 4; ++j) {
-                                const float h0 = __bfloat162float(__float2bfloat16_rn(v[2 * j])), h1 = __bfloat162float(__float2bfloat16_rn(v[2 * j + 1]));
-                                hw[j] = pack_bf16(v[2 * j], v[2 * j + 1]);
-                                lw[j] = pack_bf16(v[2 * j] - h0, v[2 * j + 1] - h1);
-                            }
-                            __nv_bfloat16* o = p.out_split + (long long)grow * p.out_pitch + c0 + g8 * 8;
-                            *reinterpret_cast<uint4*>(o) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                            *reinterpret_cast<uint4*>(o + p.out_lo) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+                        for (int j = 0; j < 4; ++j) {
+                            const float h0 = __bfloat162float(__float2bfloat16_rn(v[2 * j])), h1 = __bfloat162float(__float2bfloat16_rn(v[2 * j + 1]));
+                            hw[j] = pack_bf16(v[2 * j], v[2 * j + 1]);
+                            lw[j] = pack_bf16(v[2 * j] - h0, v[2 * j + 1] - h1);
                         }
-                        if (p.out_f32) {
-                            float* o = p.out_f32 + (size_t)grow * COUT + c0 + g8 * 8;
-                            stg_f4(o, make_float4(v[0], v[1], v[2], v[3]));
-                            stg_f4(o + 4, make_float4(v[4], v[5], v[6], v[7]));
-                        }
+                        __nv_bfloat16* o = p.out_split + (long long)grow * p.out_pitch + c0 + g8 * 8;
+                        *reinterpret_cast<uint4*>(o) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
+                        *reinterpret_cast<uint4*>(o + p.out_lo) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+                    }
+                    if (p.out_f32) {
+                        float* o = p.out_f32 + (size_t)grow * COUT + c0 + g8 * 8;
+                        stg_f4(o, make_float4(v[0], v[1], v[2], v[3]));
+                        stg_f4(o + 4, make_float4(v[4], v[5], v[6], v[7]));
                     }
                 }
             }
-            tc_fence_before();
-            mbar_arrive(bar_tempty + 8 * acc);
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 4) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
     }
 }
 
 template <int CIN, int COUT>
 int launch_spt(const SptP& p, const void* w_packed, cudaStream_t st) {
-    constexpr int STAGES = (COUT >= 128) ? 3 : 4;
+    constexpr int STAGES = (COUT >= 128) ? 2 : (COUT >= 64 ? 3 : 4);
     constexpr int B_BYTES = 2 * COUT * 128;
-    constexpr size_t SMEM = (size_t)STAGES * (2 * SPT_ATILE + B_BYTES) + SPT_M * 28 * 4 + 512;
+    constexpr size_t SMEM = (size_t)STAGES * (2 * SPT_ATILE + B_BYTES) + (size_t)SPT_M * (COUT < 64 ? COUT : 64) * 4 + SPT_M * 28 * 4 + 512;
     static_assert(SMEM <= 227 * 1024, "shared memory budget");
     PFN_tmEncodeTiled enc = get_encode();
     if (!enc) return HEAL_ERR_DRIVER;

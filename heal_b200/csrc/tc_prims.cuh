@@ -1,5 +1,5 @@
-// tcgen05 / TMA / mbarrier primitives shared by the tensor-core kernels (conv2d_tc.cu, conv3x3_ring.cu, spconv_tc.cu).
-// Inline PTX for sm_100a; every helper is a thin wrapper around ONE instruction (or a bounded wait loop).
+// wgmma / TMA / mbarrier primitives shared by the tensor-core kernels (conv2d_tc.cu, conv3x3_ring.cu, spconv_tc.cu).
+// Inline PTX for sm_90a; every helper is a thin wrapper around ONE instruction (or a bounded wait loop).
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
@@ -49,71 +49,114 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
                  ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
 
-// K-major, 128B-swizzled shared-memory matrix descriptor (sm_100): rows of 128 B, 8-row groups 1024 B apart.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
+// K-major, 128B-swizzled shared-memory matrix descriptor (sm_90 wgmma): rows of 128 B, 8-row groups 1024 B apart.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr & 0x3FFFF) >> 4);          // start address (16 B units)
     d |= (uint64_t)1 << 16;                           // leading byte offset (unused for swizzled K-major) = 1
     d |= (uint64_t)(1024 >> 4) << 32;                 // stride byte offset: 8 rows * 128 B
-    d |= (uint64_t)1 << 46;                           // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;                           // SWIZZLE_128B
+    d |= (uint64_t)1 << 62;                           // SWIZZLE_128B
     return d;
 }
 
 // K-major, 32B-swizzled descriptor (rows of 32 B = 16 bf16, 8-row groups 256 B apart): the packed diagonal weight sub-blocks.
-__device__ __forceinline__ uint64_t umma_desc_sw32(uint32_t saddr) {
+__device__ __forceinline__ uint64_t gmma_desc_sw32(uint32_t saddr) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
     d |= (uint64_t)1 << 16;
     d |= (uint64_t)(256 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)6 << 61;                           // SWIZZLE_32B
+    d |= (uint64_t)3 << 62;                           // SWIZZLE_32B
     return d;
 }
 
-// Same, for a start address that is only 128 B aligned (a ROW offset inside a TMA-written swizzled tile).
-// Measured on B200 (profiles/halo_diag.py): the tensor core applies the 128B swizzle to the ABSOLUTE shared-memory
-// address (bits [4,7) ^= bits [7,10)), exactly like the TMA unit, so a row-shifted view needs no base-offset:
-// the descriptor's base_offset field must stay 0 (setting it to the row phase produces garbage).
-__device__ __forceinline__ uint64_t umma_desc_sw128_off(uint32_t saddr, int mode) {
+// Same, for a start address that is only 128 B aligned (a ROW offset inside a TMA-written swizzled tile).  mode 0: base offset
+// 0 (the swizzle is taken from the absolute shared-memory address, as the TMA unit writes it); mode 1: base offset = the row
+// phase of the start address (HEAL_TC_BO=1, kept to check the convention on a new part).
+__device__ __forceinline__ uint64_t gmma_desc_sw128_off(uint32_t saddr, int mode) {
     uint32_t ph = (saddr >> 7) & 7;
-    uint32_t bo = (mode == 0) ? 0u : ph;      // mode 1 kept only for the diagnostic script
-    return umma_desc_sw128(saddr) | ((uint64_t)bo << 49);
+    uint32_t bo = (mode == 0) ? 0u : ph;
+    return gmma_desc_sw128(saddr) | ((uint64_t)bo << 49);
 }
 
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-    asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n"
-                 " tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}"
-                 ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
+// Warpgroup MMA, D(64 x N, fp32 registers) (+)= A(64 x 16, smem) * B(16 x N, smem), both operands K-major bf16.
+// accum == 0 overwrites D (first K step of a tile).  Fragment of thread t of the warpgroup: register i holds
+// row 16*(t/32) + (t%32)/4 + 8*((i%4)/2), column 8*(i/4) + 2*(t%4) + i%2.
+__device__ __forceinline__ void wgmma_n16(float* d, uint64_t a, uint64_t b, uint32_t accum) {
+    asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %10, 0;\n"
+                 " wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+                 : "l"(a), "l"(b), "r"(accum));
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+__device__ __forceinline__ void wgmma_n32(float* d, uint64_t a, uint64_t b, uint32_t accum) {
+    asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %18, 0;\n"
+                 " wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                 : "l"(a), "l"(b), "r"(accum));
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_n64(float* d, uint64_t a, uint64_t b, uint32_t accum) {
+    asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %34, 0;\n"
+                 " wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "l"(a), "l"(b), "r"(accum));
+}
+__device__ __forceinline__ void wgmma_n128(float* d, uint64_t a, uint64_t b, uint32_t accum) {
+    asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %66, 0;\n"
+                 " wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(a), "l"(b), "r"(accum));
+}
+template <int N>
+__device__ __forceinline__ void wgmma_bf16(float* d, uint64_t a, uint64_t b, uint32_t accum) {
+    static_assert(N == 16 || N == 32 || N == 64 || N == 128, "wgmma N");
+    if constexpr (N == 16) wgmma_n16(d, a, b, accum);
+    else if constexpr (N == 32) wgmma_n32(d, a, b, accum);
+    else if constexpr (N == 64) wgmma_n64(d, a, b, accum);
+    else wgmma_n128(d, a, b, accum);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+template <int R>
+__device__ __forceinline__ void regs_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void regs_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* v) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-                 "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                   "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-                   "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-                   "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                 : "r"(taddr) : "memory");
+// Accumulator transposition through shared memory.  The epilogues work one output ROW per thread (32 consecutive channels),
+// the wgmma fragment spreads a row over 4 lanes; a chunk of SW (16, 32 or 64) columns of the 128-row tile goes through an
+// fp32 scratch [128 rows][SW] whose 16-byte slots are XOR-swizzled by row (conflict-free row reads).
+template <int SW>
+__device__ __forceinline__ uint32_t scratch_addr(uint32_t base, int row, int col) {
+    constexpr int SWZ = (SW / 4 < 8 ? SW / 4 : 8) - 1;
+    return base + (uint32_t)(row * SW * 4) + (uint32_t)((((col >> 2) ^ (row & SWZ)) << 4) + (col & 3) * 4);
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* v) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                   "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-                 : "r"(taddr) : "memory");
+// columns [c0, c0 + SW) of the 64 x (2 * NR) fragment L (rows row0 .. row0 + 63 of the tile) -> scratch
+template <int NR, int SW>
+__device__ __forceinline__ void frag_to_scratch(const float* L, uint32_t base, int row0, int c0) {
+    const int t = threadIdx.x & 127;
+    const int r = row0 + 16 * (t >> 5) + ((t & 31) >> 2);
+#pragma unroll
+    for (int i = 0; i < NR; i += 2) {
+        const int col = 8 * (i >> 2) + 2 * (t & 3) - c0;
+        if (col >= 0 && col < SW) {
+            const int rr = r + 8 * ((i & 3) >> 1);
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(scratch_addr<SW>(base, rr, col)), "f"(L[i]), "f"(L[i + 1]) : "memory");
+        }
+    }
 }
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// N (multiple of 4) consecutive fp32 of one scratch row, starting at chunk column col -> raw bits
+template <int SW, int N>
+__device__ __forceinline__ void scratch_row(uint32_t base, int row, int col, uint32_t* raw) {
+#pragma unroll
+    for (int j = 0; j < N; j += 4) {
+        asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
+                         : "=r"(raw[j]), "=r"(raw[j + 1]), "=r"(raw[j + 2]), "=r"(raw[j + 3]) : "r"(scratch_addr<SW>(base, row, col + j)) : "memory");
+    }
+}
 
-// One lane of a converged warp; the compiler keeps code under this predicate on the uniform datapath (the tcgen05 /
-// TMA instructions take uniform-register operands: issuing them from an `if (lane == 0)` region instead costs an
-// ELECT + branch loop per instruction, measured at ~110 cycles per tcgen05.mma).
+// One lane of a converged warp; the compiler keeps code under this predicate on the uniform datapath (the TMA
+// instructions take uniform-register operands: issuing them from an `if (lane == 0)` region costs an ELECT + branch loop
+// per instruction).
 __device__ __forceinline__ uint32_t elect_one() {
     uint32_t pred = 0;
     asm volatile("{\n .reg .b32 rx;\n .reg .pred px;\n elect.sync rx|px, 0xffffffff;\n @px mov.s32 %0, 1;\n}" : "+r"(pred));
@@ -129,6 +172,7 @@ template <int N>
 __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// named barrier over the 256 threads of the two consumer warpgroups
 __device__ __forceinline__ void epi_bar(int id) { asm volatile("bar.sync %0, 256;" ::"r"(id) : "memory"); }
 
 __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {

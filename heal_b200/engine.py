@@ -1,5 +1,5 @@
 """Execution helpers shared by the mirror modules: precision mode, parameter folding/packing cache and
-the conv dispatcher (tcgen05 implicit GEMM where eligible, fp32 CUDA-core kernel otherwise).
+the conv dispatcher (wgmma implicit GEMM where eligible, fp32 CUDA-core kernel otherwise).
 
 Parameters stay ordinary nn.Parameters with the reference's state-dict key names
 (SURVEY.md 8b "Parameters / ownership"); what the kernels consume is a *derived* cache (BN folded in
@@ -7,7 +7,7 @@ fp64, weights re-laid out for the kernels) that is rebuilt whenever a source ten
 changes (load_state_dict / optimizer step) or the module moves device.
 
 Precision modes (set_precision):
-  'tc32'  (default) dense stride-1 convs on tcgen05 with split-bf16 operands (3 MMAs / K-step, fp32
+  'tc32'  (default) dense stride-1 convs on wgmma with split-bf16 operands (3 MMAs / K-step, fp32
           accumulate: fp32-equivalent, meets the 1e-3 parity bar); activations stored as split-bf16.
   'bf16'  same kernels, activations stored as ONE bf16 plane, weights keep both planes (a_hi x [b_hi | b_lo]: the weights are
           not rounded to 8 mantissa bits, only the activations are; 1e-2 parity bar, BASELINE config 4).  HEAL_BF16_WEIGHTS=1

@@ -135,8 +135,8 @@ class FrameInterleaver:
 class FramePipeline:
     """Two captured frames on four streams: while frame i computes, frame i+1's inputs are copied in (pinned host -> HBM), frame
     i-1's predictions are copied out (HBM -> pinned host), and -- each frame slot replays on its OWN compute stream -- the head of
-    frame i+1 (voxeliser, VFE, stem: small latency-bound kernels) runs in the gaps of frame i's convolutions (measured +10 %
-    frames/s over one compute stream; `compute_streams=1` restores strict frame-after-frame execution).  The serving loop's
+    frame i+1 (voxeliser, VFE, stem: small latency-bound kernels) runs in the gaps of frame i's convolutions
+    (`compute_streams=1` restores strict frame-after-frame execution).  The serving loop's
     public entry point:
 
         pipe = FramePipeline(model, n_agents, point_capacity, pairwise_shape)

@@ -90,7 +90,7 @@ class CamEncode_Resnet101(nn.Module):
     names -> same state-dict keys (the torchvision modules are parameter containers).  `heads_nhwc` runs the whole trunk on
     the conv engine (SURVEY.md 8f-2):
       conv1 7x7/2 + bn1 + ReLU   as a 3x3 convolution on the 4x4 space-to-depth image (3 -> 64 input channels, 4 output phases
-                                 x 64 channels): a tcgen05 shape instead of a K = 3 stem; exact re-indexing of the same sums
+                                 x 64 channels): a wgmma shape instead of a K = 3 stem; exact re-indexing of the same sums
       maxpool 3x3/2              heal_maxpool3x3s2 reading the phase-major stem output directly
       layer1, layer2             torchvision Bottlenecks: 1x1 / 3x3 (stride) / 1x1 + residual, each conv+BN(+ReLU) one kernel
       depth_head | image_head    one fused 1x1 convolution 512 -> D + C, fp32 channels-last output

@@ -2,9 +2,8 @@
 
 Only the parameter containers keep the reference's shape -- the checkpoint keys are `layers.<i>.double_conv.{0,2}.{weight,bias}`, so
 the two convolutions must sit at indices 0 and 2 of a Sequential called `double_conv`.  Nothing in that Sequential is ever called:
-both 3x3 convolutions (bias + ReLU folded) go through `engine.conv_bn_act`, i.e. the tcgen05 implicit-GEMM kernel on channels-last
-split-bf16 activations; these two launches are the MMA-bound ones of the frame (384->256 and 256->256 on the 256 x 256 fused map,
-~94 % of the sustained tensor peak).  `forward_nhwc` is the engine-internal entry (Act in, Act out); `forward` keeps the reference's
+both 3x3 convolutions (bias + ReLU folded) go through `engine.conv_bn_act`, i.e. the wgmma implicit-GEMM kernel on channels-last
+split-bf16 activations; these two launches are the MMA-bound ones of the frame (384->256 and 256->256 on the 256 x 256 fused map).  `forward_nhwc` is the engine-internal entry (Act in, Act out); `forward` keeps the reference's
 NCHW tensor signature for callers outside the engine."""
 import torch.nn as nn
 

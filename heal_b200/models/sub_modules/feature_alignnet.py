@@ -5,7 +5,7 @@ ConvNeXtBlock (feature_alignnet_modules.py:299-345): dwconv 7x7 -> LayerNorm(cha
 GELU -> Linear(4 dim, dim) -> gamma -> + input.  The nn modules below only hold the parameters under the reference's state-dict
 names; per block the compute is three kernels on channels-last `Act`s:
   heal_dwconv_layernorm                         depthwise conv + bias + LayerNorm, one HBM pass
-  heal_conv2d_tc 1x1 dim -> 4 dim, GELU         (pwconv1 as a 1x1 convolution on tcgen05, erf GELU in the epilogue)
+  heal_conv2d_tc 1x1 dim -> 4 dim, GELU         (pwconv1 as a 1x1 convolution on wgmma, erf GELU in the epilogue)
   heal_conv2d_tc 1x1 4 dim -> dim + residual    (pwconv2 with gamma folded into weight and bias, block input as the residual)
 The other aligners of the reference (scaligner, resnet1x1/3x3, sdta, cbam, fanet) are not used by any HEAL yaml and raise."""
 import torch

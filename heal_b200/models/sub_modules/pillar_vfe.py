@@ -1,4 +1,4 @@
-"""PillarVFE on the fused sm_100a kernel (heal_pillar_vfe_scatter).
+"""PillarVFE on the fused sm_90a kernel (heal_pillar_vfe_scatter).
 
 Mirror of opencood/models/sub_modules/pillar_vfe.py: same class names, ctor arguments, state-dict keys
 (`pfn_layers.0.linear.weight`, `pfn_layers.0.norm.*`) and `forward(batch_dict)` contract

@@ -116,9 +116,9 @@ class ResNetModified(nn.Module):
 
     # A level whose largest per-layer tensor (all images) exceeds this is run image by image ("agent-major"): each agent
     # goes through the whole level before the next one starts, so that its intermediates (<= 34 MB at 256x256) stay
-    # resident in the 126 MB L2 between producer and consumer instead of round-tripping HBM.
-    # Off by default: on B200 the extra launches (fixed ~7 us each) cost more than the L2 residency saved (measured
-    # 7.4 ms/frame agent-major vs 5.9 ms batched, profiles/); set HEAL_AGENT_MAJOR_MB to experiment.
+    # resident in L2 (50 MB on the H100) between producer and consumer instead of round-tripping HBM.
+    # Off by default: on the B200 build it was first tried on, the extra launches cost more than the L2 residency saved; it has
+    # not been measured on the H100.  Set HEAL_AGENT_MAJOR_MB to experiment.
     AGENT_MAJOR_BYTES = (int(__import__('os').environ.get('HEAL_AGENT_MAJOR_MB', '0')) << 20) or (1 << 62)
 
     def _run_level(self, layer, x, out=None):

@@ -6,7 +6,7 @@ that is not on a CUDA device raises.
 
 Activations travel between kernels as `Act` objects: channels-last buffers in one of three storage
 formats — 'f32' (N,H,W,C) fp32; 'bf16' (1,N,H,W,C) bf16; 'split' (2,N,H,W,C) bf16 planes (hi, lo) with
-x ~= hi + lo (16 mantissa bits), the operand format of the tcgen05 fp32-equivalent convolution.
+x ~= hi + lo (16 mantissa bits), the operand format of the wgmma fp32-equivalent convolution.
 At module boundaries feature maps are *logically* (N,C,H,W) fp32 torch tensors that are *physically*
 channels-last (`x.permute(0,2,3,1)` contiguous), which keeps the reference's shapes at zero cost.
 """
@@ -429,7 +429,7 @@ def _coutp(cout: int) -> int:
 
 
 class PackedConvTC:
-    """Folded + packed split-bf16 parameters for heal_conv2d_tc (tcgen05 path)."""
+    """Folded + packed split-bf16 parameters for heal_conv2d_tc (wgmma path)."""
 
     def __init__(self, w, bias, kh, kw, pad, cin, cout, coutp, relu, up, planes, stride=1, blockdiag=False, groups=1):
         self.w, self.bias = w, bias
@@ -549,7 +549,7 @@ def conv2d_simt(x: Act, pc: PackedConv, residual: Optional[Act] = None, out: Opt
 def conv2d_tc(x: Act, pc: PackedConvTC, residual: Optional[Act] = None, out: Optional[Act] = None,
               out_coffset: int = 0, in_coffset: int = 0, want_split: bool = True,
               out_f32: Optional[Act] = None, want_f32: bool = False, out32_coffset: int = 0):
-    """tcgen05 conv.  x: Act 'split' (planes 2) or 'bf16' (planes 1).  Returns (Act split/bf16 | None, Act f32 | None)."""
+    """wgmma conv.  x: Act 'split' (planes 2) or 'bf16' (planes 1).  Returns (Act split/bf16 | None, Act f32 | None)."""
     _need_cuda(pc.w)
     assert x.planes in (1, 2) and pc.planes >= x.planes      # weights may carry a lo plane the activations do not ('bf16' mode)
     N, H, W = x.N, x.H, x.W
@@ -953,9 +953,9 @@ def pillar_vfe_sparse(voxel_features, voxel_num_points, voxel_coords, w_folded, 
     return SparseCanvas(pf, idmap, batch_size, ny, nx, densify, feats_split=fsplit)
 
 
-# The stem as two tcgen05 gather-GEMMs (heal_stem_rulebook + heal_spconv_gather_gemm_tc with planar I/O) instead of k_sparse_stem.
-# Correct and tested, but measured SLOWER on the C2 frame (0.36 ms vs 0.20 ms: 2 560 output tiles x up to 9 K-blocks of mostly
-# zero-filled rows, weights re-streamed per tile) -> opt-in; the fp32 gather kernel stays the default.
+# The stem as two wgmma gather-GEMMs (heal_stem_rulebook + heal_spconv_gather_gemm_tc with planar I/O) instead of k_sparse_stem.
+# Correct and tested, but slower on the C2 frame on the B200 build it was first measured on (2 560 output tiles x up to 9 K-blocks
+# of mostly zero-filled rows, weights re-streamed per tile) -> opt-in; the fp32 gather kernel stays the default.
 STEM_GATHER_TC = False
 
 

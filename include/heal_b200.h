@@ -1,4 +1,4 @@
-/* heal_b200 — C ABI of the B200-native (sm_100a) per-frame perception hot path of HEAL / OpenCOOD.
+/* heal_b200 — C ABI of the H100-native (sm_90a) per-frame perception hot path of HEAL / OpenCOOD.
  *
  * The reference (yifanlu0227/HEAL) is pure Python/PyTorch on this path and has NO foreign-function
  * interface of its own; each entry point below therefore cites the reference *Python* call site it
@@ -40,7 +40,7 @@ typedef struct {
     size_t plane_stride;
 } heal_act_t;
 int heal_abi_version(void);
-/* sm_100a build check: returns 0 when a Blackwell (cc 10.x) device is current, negative otherwise. */
+/* sm_90a build check: returns 0 when a Hopper (cc 9.x) device is current, negative otherwise. */
 int heal_device_check(void);
 /* number of kernels this library has launched in this process so far */
 long long heal_launch_count(void);
@@ -120,8 +120,8 @@ int heal_conv2d_simt(const heal_act_t* in, int N, int H, int W, int Cin,
                      const heal_act_t* residual, const heal_act_t* out, int Ho, int Wo, int Cout,
                      int upsample, int up_i, int up_j, int relu, void* stream);
 
-/* ---- 2-D convolution, tcgen05 tensor-core path ---------------------------------------------------
- * Same reference ops as heal_conv2d_simt, evaluated as an implicit GEMM with tcgen05.mma (TMEM
+/* ---- 2-D convolution, wgmma tensor-core path ---------------------------------------------------
+ * Same reference ops as heal_conv2d_simt, evaluated as an implicit GEMM with wgmma (register
  * accumulators) fed by TMA.  Activations are "split-bf16": `planes` bf16 channels-last planes
  * (planes=2: hi = bf16(x), lo = bf16(x-hi), fp32-equivalent via the three products a_hi*b_hi + a_hi*b_lo + a_lo*b_hi per K
  * step; planes=1: plain bf16).
@@ -234,7 +234,7 @@ int heal_spconv_gather_gemm(const float* in_feats, const int* nbr, const int* ou
                             const float* weight, const float* bias, int c_in, int c_out, int relu,
                             float* out_feats, void* stream);
 
-/* The same gather-GEMM on the tensor cores (csrc/spconv_tc.cu: tcgen05.mma, TMEM accumulators, cp.async row gather into
+/* The same gather-GEMM on the tensor cores (csrc/spconv_tc.cu: wgmma, register accumulators, cp.async row gather into
  * 128B-swizzled K-major tiles, TMA weight tiles), for c_in in {16,32,64}.  Features are "split rows": (rows, 2*C) bf16 =
  * [hi C | lo C] with x ~= hi + lo; products a_hi*b_hi + a_hi*b_lo + a_lo*b_hi, fp32 accumulation (fp32-equivalent).
  *   w_packed   [2 planes][KB * c_out rows][64] bf16, KB = ceil(kvol / (64 / c_in)); column = (offset within K-block) * c_in + ci

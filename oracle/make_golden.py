@@ -10,7 +10,7 @@ import sys
 import numpy as np
 import torch
 
-from oracle import ref_shim, procedural, voxelizer
+from oracle import golden, ref_shim, procedural, voxelizer
 
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden")
 
@@ -105,7 +105,7 @@ def main():
         # intermediate: encoder + backbone features, for finer-grained parity
         enc = model.encoder_m1(copy.deepcopy(data), "m1")
         bb = model.backbone_m1({"spatial_features": enc})["spatial_features_2d"]
-    torch.save({
+    golden.save({
         "args": args, "shapes": shapes, "data": data,
         "out": {"cls_preds": out["cls_preds"], "reg_preds": out["reg_preds"], "dir_preds": out["dir_preds"],
                 "occ_single_list": out["occ_single_list"]},
@@ -122,7 +122,7 @@ def main():
         w = warp_affine_simple(x, aff[0, 0, :3], (24, 40))
         w_ac = warp_affine_simple(x, aff[0, 0, :3], (24, 40), align_corners=True)
         att = AttFusion(128)(x, torch.tensor([3]), aff)
-    torch.save({"x": x, "pairwise_t_matrix": data["pairwise_t_matrix"], "H": 9.6, "W": 16.0, "affine": aff,
+    golden.save({"x": x, "pairwise_t_matrix": data["pairwise_t_matrix"], "H": 9.6, "W": 16.0, "affine": aff,
                 "warp_s": w[:, ::8].contiguous(), "warp_align_corners_s": w_ac[:, ::8].contiguous(), "att": att}, os.path.join(OUT, "warp_att.pt"))
     print("warp_att:", tuple(w.shape), tuple(att.shape))
 
@@ -135,7 +135,7 @@ def main():
     xin = torch.randn(2, 64, 32, 48, generator=g)
     with torch.no_grad():
         y = bbm({"spatial_features": xin})["spatial_features_2d"]
-    torch.save({"cfg": cfg, "shapes": bshapes, "x": xin, "y_s": y[:, ::4].contiguous()}, os.path.join(OUT, "base_bev_backbone_small.pt"))
+    golden.save({"cfg": cfg, "shapes": bshapes, "x": xin, "y_s": y[:, ::4].contiguous()}, os.path.join(OUT, "base_bev_backbone_small.pt"))
     print("base_bev_backbone_small:", tuple(y.shape))
     # ---- 4. Lift-Splat-Shoot geometry + voxel pooling (reference methods on a ctor-less instance) ------
     from opencood.models.heter_encoders import LiftSplatShoot
@@ -164,7 +164,7 @@ def main():
         new_x = torch.softmax(depth_logits, dim=1).unsqueeze(1) * feat.unsqueeze(2)        # lss_submodule.py:228-229
         xx = new_x.view(Bn, Nc, Cc, D, fH, fW).permute(0, 1, 3, 4, 5, 2)                   # heter_encoders.py:156-157
         bev = obj.voxel_pooling(geom, xx)
-    torch.save({"cfg": lcfg, "rots": rots, "trans": trans, "intrins": intr, "post_rots": post_rots, "post_trans": post_trans,
+    golden.save({"cfg": lcfg, "rots": rots, "trans": trans, "intrins": intr, "post_rots": post_rots, "post_trans": post_trans,
                 "depth_logits": depth_logits, "feat": feat, "geom": geom, "bev": bev}, os.path.join(OUT, "lss_small.pt"))
     print("lss_small:", tuple(geom.shape), tuple(bev.shape), float(bev.abs().max()))
     # ---- 5. HeterModelBaseline + AttFusion (C3 family; PointPillar encoder so that the reference runs without spconv) ----
@@ -175,7 +175,7 @@ def main():
     bm.load_state_dict(procedural.make_state_dict(bshapes2), strict=True)
     with torch.no_grad():
         bout = bm(copy.deepcopy(data))
-    torch.save({"args": bargs, "shapes": bshapes2, "data": data,
+    golden.save({"args": bargs, "shapes": bshapes2, "data": data,
                 "out": {k: bout[k] for k in ("cls_preds", "reg_preds", "dir_preds")}},
                os.path.join(OUT, "heter_model_baseline_att_small.pt"))
     print("heter_model_baseline_att_small:", {k: tuple(v.shape) for k, v in bout.items() if torch.is_tensor(v)})
@@ -281,7 +281,7 @@ def make_postprocess_golden():
                                         {"ego": {"cls_preds": cls.clone(), "reg_preds": reg.clone(), "dir_preds": dirp.clone(), "iou_preds": iou.clone()}})
     multi["iou"] = {"cavs": [{"cls": cls, "reg": reg, "dir": dirp, "iou": iou, "T": T}], "boxes": boxes, "scores": scores}
     print("postprocess iou -> kept", boxes.shape[0])
-    torch.save({"params": params, "anchors": anchors, "cases": cases, "multi": multi}, os.path.join(OUT, "postprocess.pt"))
+    golden.save({"params": params, "anchors": anchors, "cases": cases, "multi": multi}, os.path.join(OUT, "postprocess.pt"))
 
 
 if __name__ == "__main__":

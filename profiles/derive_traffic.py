@@ -68,7 +68,7 @@ def main():
             d["kernels"].add(m.group(1) if m else l["name"][:40])
         i += n
     tot_us = sum(d["us_under_ncu"] for d in fam.values()) or 1.0
-    tc = [l for l in frame if "k_conv2d_tc" in l["name"] or "k_gconv3x3_ring" in l["name"]]      # the tcgen05 dense-map convolutions
+    tc = [l for l in frame if "k_conv2d_tc" in l["name"] or "k_gconv3x3_ring" in l["name"]]      # the wgmma dense-map convolutions
     out = {
         "source": f"{os.path.basename(src)} + {os.path.basename(seqf)}: ncu --metrics gpu__time_duration.sum,dram__bytes_read.sum,"
                   "dram__bytes_write.sum --clock-control none, python profiles/ncu_frame.py, last eager frame; cold-cache, serialised",

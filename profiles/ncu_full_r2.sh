@@ -17,7 +17,7 @@ cap() {  # name, kernel regex, extra ncu args..., -- , python args
 }
 # C2: the HBM-bound named ops (every launch of one eager frame)
 cap c2_small "k_pillar_vfe_scatter|k_select|k_cells_insert|k_pyramid_fuse|k_sparse_stem|k_fill_idmap" -- --workload c2 --frames 1
-# C2: the tcgen05 conv, first 26 launches (per-agent ResNet + ResNeXt level 0 + start of level 1) and the tail (deblocks, shrink, heads)
+# C2: the wgmma conv, first 26 launches (per-agent ResNet + ResNeXt level 0 + start of level 1) and the tail (deblocks, shrink, heads)
 cap c2_conv_head "k_conv2d_tc" --launch-count 26 -- --workload c2 --frames 1
 cap c2_conv_tail "k_conv2d_tc" --launch-skip 49 --launch-count 8 -- --workload c2 --frames 1
 # C3: tensor-core sparse conv, rulebooks, AttFusion, HeightCompression

@@ -7,7 +7,7 @@ import subprocess
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB = os.path.join(HERE, "..", "heal_b200", "libheal_b200.so")
-OPS = ["UTCHMMA", "UTCBAR", "LDTM", "UTCCP", "UTMALDG", "UTMASTG", "LDGSTS", "HMMA"]
+OPS = ["HGMMA", "UTMALDG", "UTMASTG", "LDGSTS", "HMMA"]
 
 
 def main():
@@ -29,8 +29,8 @@ def main():
             if op in OPS:
                 per[cur][op] += 1
                 total[op] += 1
-    out = ["# SASS instruction counts of heal_b200/libheal_b200.so (cuobjdump -sass, sm_100a), kernels that use the tensor-core / TMA / async-copy paths",
-           "# UTCHMMA = tcgen05.mma (kind::f16), LDTM = tcgen05.ld, UTCBAR = tcgen05.commit, UTMALDG / UTMASTG = TMA tensor load / store, LDGSTS = cp.async, HMMA = mma.sync",
+    out = ["# SASS instruction counts of heal_b200/libheal_b200.so (cuobjdump -sass, sm_90a), kernels that use the tensor-core / TMA / async-copy paths",
+           "# HGMMA = wgmma.mma_async, UTMALDG / UTMASTG = TMA tensor load / store, LDGSTS = cp.async, HMMA = mma.sync",
            "total: " + ", ".join(f"{k}={total[k]}" for k in sorted(OPS))]
     for name, c in per.items():
         if c:

@@ -1,4 +1,4 @@
-"""Timing experiment for the tcgen05 conv: where does a tile's time go?  HEAL_TC_DBG bits (results invalid, timing only):
+"""Timing experiment for the wgmma conv: where does a tile's time go?  HEAL_TC_DBG bits (results invalid, timing only):
 1 = skip the epilogue's global stores, 2 = skip the weight (B) TMA loads, 4 = skip the activation (A) TMA loads,
 8 = skip the residual loads, 16 = skip the MMAs."""
 import os

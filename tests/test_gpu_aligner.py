@@ -6,6 +6,8 @@ import os
 import pytest
 import torch
 
+from oracle import golden
+
 from workloads import procedural
 
 pytestmark = pytest.mark.gpu
@@ -24,7 +26,7 @@ def test_convnext_aligner_vs_reference_golden(golden_dir, prec, tol):
     from heal_b200 import engine
     from heal_b200.models.sub_modules.feature_alignnet import AlignNet
     engine.set_precision(prec)
-    g = torch.load(os.path.join(golden_dir, "convnext_aligner.pt"), weights_only=False)
+    g = golden.load(os.path.join(golden_dir, "convnext_aligner.pt"))
     m = AlignNet(copy.deepcopy(g["cfg"])).eval()
     assert procedural.shapes_of(m) == g["shapes"]                  # same state-dict keys and shapes as the reference module
     m.load_state_dict(procedural.make_state_dict(g["shapes"]), strict=True)
@@ -75,7 +77,7 @@ def test_heter_pyramid_collab_with_convnext_aligner_vs_oracle():
     sd = procedural.make_state_dict(procedural.shapes_of(m))
     m.load_state_dict(sd, strict=True)
     m = m.cuda()
-    g = torch.load(os.path.join(os.path.dirname(__file__), "golden", "heter_pyramid_collab_small.pt"), weights_only=False)
+    g = golden.load(os.path.join(os.path.dirname(__file__), "golden", "heter_pyramid_collab_small.pt"))
     data = g["data"]
     with torch.no_grad():
         ref = nets.heter_pyramid_collab(sd, args, copy.deepcopy(data))

@@ -16,6 +16,8 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import golden
+
 from oracle import make_golden, nets, ref_shim
 from oracle import postprocess as opp
 from workloads import procedural
@@ -55,7 +57,7 @@ def test_reference_callers_drive_the_b200_path(golden_dir):
     assert "opencood.models.heter_pyramid_collab" in done
     from opencood.tools.train_utils import create_model
     from opencood.tools import inference_utils
-    g = torch.load(os.path.join(golden_dir, "heter_pyramid_collab_small.pt"), weights_only=False)
+    g = golden.load(os.path.join(golden_dir, "heter_pyramid_collab_small.pt"))
     rng_ = list(g["args"]["lidar_range"])
     params = make_golden.postprocess_params(rng=tuple(rng_))
     params["target_args"]["score_threshold"] = 0.5
@@ -116,7 +118,7 @@ def test_postprocessor_subclass_falls_back_to_the_reference_for_cpu_and_late_fus
     _install_reference_with_quad_polygon()
     from heal_b200 import install
     cls = install.install_gpu_postprocessor()
-    gold = torch.load(os.path.join(golden_dir, "postprocess.pt"), weights_only=False)
+    gold = golden.load(os.path.join(golden_dir, "postprocess.pt"))
     pp = cls(copy.deepcopy(gold["params"]), train=False)
     c = gold["cases"]["sparse"]
     data = {"ego": {"transformation_matrix": c["T"], "anchor_box": gold["anchors"]}}

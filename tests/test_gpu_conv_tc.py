@@ -1,4 +1,4 @@
-"""tcgen05 implicit-GEMM conv (heal_conv2d_tc) vs PyTorch CPU fp32, ordered from a bare GEMM tile to full features.
+"""wgmma implicit-GEMM conv (heal_conv2d_tc) vs PyTorch CPU fp32, ordered from a bare GEMM tile to full features.
 fp32-equivalent (split-bf16, planes=2) must meet 1e-3 (typically ~2e-5); bf16 (planes=1) must meet 1e-2 relative to scale."""
 import pytest
 import torch

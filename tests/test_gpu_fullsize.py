@@ -1,8 +1,9 @@
 """Full-size parity: the BASELINE.json configs at their real shapes (range +-102.4 m -> 512x512 pillars / 2048x2048x40 voxels,
-256x256 fusion map, 64-line clouds, 704x256 images), CUDA path vs the UNMODIFIED reference modules on CPU (C1, C2: oracle/_ref
-through oracle.ref_runner) or the oracle port (C3 SECOND: no spconv-free reference; C4: the reference's LiftSplatShoot constructor
+256x256 fusion map, 64-line clouds, 704x256 images), CUDA path vs the UNMODIFIED reference modules on CPU (C1, C2: seeded
+samples of the reference heads stored by oracle/make_golden_fullsize.py in tests/golden/fullsize_c*.npz) or the oracle port (C3 SECOND: no spconv-free reference; C4: the reference's LiftSplatShoot constructor
 hard-codes CUDA).  Tolerances are north_star's: 1e-3 (fp32-equivalent tc32) and 1e-2 (bf16), relative to max(1, max|ref|)."""
 import copy
+import os
 
 import numpy as np
 import pytest
@@ -32,6 +33,24 @@ def _check(out, ref, tol, tag):
         assert err <= tol * scale, (tag, k, err, scale)
 
 
+def _check_golden(out, gold, tol, tag):
+    """out vs the stored reference sample: same shapes, and every sampled element within tol * max(1, max|ref|)."""
+    for k in HEADS:
+        g = out[k].float().cpu()
+        assert tuple(g.shape) == tuple(gold[f"{k}.shape"]), (tag, k, g.shape, gold[f"{k}.shape"])
+        idx = torch.from_numpy(gold[f"{k}.index"].astype(np.int64))
+        r = torch.from_numpy(gold[f"{k}.value"])
+        err = (g.reshape(-1)[idx] - r).abs().max().item()
+        scale = max(float(gold[f"{k}.max_abs"]), 1.0)
+        print(f"{tag}/{k}: max|ref|={scale:.3f} max_abs_err={err:.3e} over {idx.numel()} sampled elements (tol {tol * scale:.3e})")
+        assert err <= tol * scale, (tag, k, err, scale)
+
+
+def _golden(name):
+    with np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", name)) as z:
+        return {k: z[k] for k in z.files}
+
+
 def _scene(n_agents, rings=64, azimuth=1024, seed=321):
     sc = synth.scene(seed, n_agents=n_agents, max_cav=max(5, n_agents), rings=rings, azimuth=azimuth)
     pts = np.concatenate(sc["points"]).astype(np.float32)
@@ -41,14 +60,14 @@ def _scene(n_agents, rings=64, azimuth=1024, seed=321):
 
 @pytest.fixture(scope="module")
 def c2_reference():
-    """One full-size 5-agent frame through the unmodified reference HeterPyramidCollab on CPU (~10 s)."""
-    from oracle import ref_runner
-    assert ref_runner.available(), "oracle/_ref missing: python -m oracle.build_ref (build container)"
-    sc, pts, offs = _scene(5)
-    model, sd = ref_runner.build_model("heter_pyramid_collab", wcfg.c2_args())
-    data, _ = ref_runner.c2_data({"clouds": sc["points"], "pairwise": sc["pairwise_t_matrix"]}, 5)
-    ref = ref_runner.forward(model, data)
-    return sc, pts, offs, sd, {k: ref[k] for k in HEADS}
+    """One full-size 5-agent frame of the unmodified reference HeterPyramidCollab (stored sample) and its inputs."""
+    from oracle import make_golden_fullsize as mgf
+    from heal_b200.models.heter_pyramid_collab import HeterPyramidCollab
+    sc = mgf.c2_scene()
+    pts = torch.from_numpy(np.concatenate(sc["points"]).astype(np.float32)).cuda()
+    offs = torch.from_numpy(np.concatenate([[0], np.cumsum([p.shape[0] for p in sc["points"]])]).astype(np.int32)).cuda()
+    sd = procedural.make_state_dict(procedural.shapes_of(HeterPyramidCollab(wcfg.c2_args())))
+    return sc, pts, offs, sd, _golden("fullsize_c2.npz")
 
 
 BF16_TOL = 2.5e-2      # see tests/test_gpu_models.py: bf16 storage noise through ~60 stored tensors; tc32 is the 1e-3 path
@@ -67,26 +86,25 @@ def test_c2_full_size_vs_unmodified_reference(c2_reference, prec, tol):
             "pairwise_t_matrix": torch.from_numpy(sc["pairwise_t_matrix"]).cuda()}
     with torch.no_grad():
         out = m(data)
-    _check(out, ref, tol, f"C2-full/{prec}")
+    _check_golden(out, ref, tol, f"C2-full/{prec}")
 
 
 def test_c1_full_size_vs_unmodified_reference():
     """configs[0]: models/point_pillar.py, one 20k-ray cloud, range +-102.4 m (512x512 pillars)."""
-    from oracle import ref_runner
+    from oracle import make_golden_fullsize as mgf
     from heal_b200 import engine
     from heal_b200.models.point_pillar import PointPillar
     engine.set_precision("tc32")
-    cloud = synth.lidar_cloud(np.random.default_rng(77), rings=20, azimuth=1000)
-    rm, sd = ref_runner.build_model("point_pillar", wcfg.c1_args())
-    data, _ = ref_runner.c1_data(cloud)
-    ref = ref_runner.forward(rm, data)
+    cloud = mgf.c1_cloud()
+    ref = _golden("fullsize_c1.npz")
     m = PointPillar(wcfg.c1_args()).eval()
+    sd = procedural.make_state_dict(procedural.shapes_of(m))
     m.load_state_dict(sd, strict=True)
     m = m.cuda()
     offs = torch.tensor([0, cloud.shape[0]], dtype=torch.int32).cuda()
     with torch.no_grad():
         out = m({"processed_lidar": {"points": torch.from_numpy(cloud).cuda(), "agent_offsets": offs}})
-    _check(out, ref, 1e-3, "C1-full/tc32")
+    _check_golden(out, ref, 1e-3, "C1-full/tc32")
 
 
 def test_c1_gpu_point_filters_equal_host_filters():

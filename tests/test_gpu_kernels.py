@@ -1,8 +1,10 @@
-"""GPU parity tests of the individual sm_100a kernels against the CPU oracle (run with -m gpu on the B200 box).
+"""GPU parity tests of the individual sm_90a kernels against the CPU oracle (run with -m gpu on an H100).
 Integer outputs are bit-exact; fp32 outputs are within 1e-3 (north_star tolerance), usually ~1e-5."""
 import numpy as np
 import pytest
 import torch
+
+from oracle import golden
 import torch.nn.functional as F
 
 from oracle import nets, voxelizer
@@ -222,7 +224,7 @@ def test_warp_att_golden(golden_dir):
     """AttFusion output of the UNMODIFIED reference (tests/golden/warp_att.pt)."""
     import os
     from heal_b200 import ops
-    g = torch.load(os.path.join(golden_dir, "warp_att.pt"), weights_only=False)
+    g = golden.load(os.path.join(golden_dir, "warp_att.pt"))
     out = ops.att_fuse(ops.to_act(g["x"].cuda()), g["affine"][0, 0, :3].cuda())
     torch.testing.assert_close(ops.act_to_nchw(out)[0].cpu().contiguous(), g["att"][0], rtol=1e-4, atol=1e-4)
 
@@ -234,7 +236,7 @@ def test_sparse_stem_equals_dense_canvas_path_and_oracle(prec):
     from heal_b200.models.sub_modules.resblock import BasicBlock, conv1x1
     from oracle import procedural
     old, old_tc, old_gather = engine.PRECISION, engine.STEM_TC, ops.STEM_GATHER_TC
-    ops.STEM_GATHER_TC = (prec == "tc32-gather")   # opt-in tcgen05 gather-GEMM stem (stem rulebook + heal_spconv_gather_gemm_tc)
+    ops.STEM_GATHER_TC = (prec == "tc32-gather")   # opt-in wgmma gather-GEMM stem (stem rulebook + heal_spconv_gather_gemm_tc)
     engine.STEM_TC = prec.endswith("-mma")          # heal_sparse_stem_tc (mma.sync, split-bf16) instead of the fp32 gather kernel
     prec = prec.split("-")[0]
     engine.set_precision(prec)
@@ -252,7 +254,7 @@ def test_sparse_stem_equals_dense_canvas_path_and_oracle(prec):
         blk.load_state_dict(blk_sd, strict=True)
         blk = blk.cuda()
         args = (col["voxel_features"], col["voxel_num_points"], col["voxel_coords"], w.cuda(), b.cuda(), PP_VOXEL, PP_RANGE, 512, 512, 2)
-        # tc32 (default engine path): PillarVFE also emits split rows and the stem runs as two tcgen05 gather-GEMMs
+        # tc32 (default engine path): PillarVFE also emits split rows and the stem runs as two wgmma gather-GEMMs
         sparse = ops.pillar_vfe_sparse(*args, want_split_rows=ops.STEM_GATHER_TC)
         _, dense = ops.pillar_vfe_scatter(*args, canvas_fmt=engine.act_fmt())
         with torch.no_grad():

@@ -5,6 +5,8 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import golden
+
 from oracle import lss
 
 pytestmark = pytest.mark.gpu
@@ -19,7 +21,7 @@ def _mats(g):
 
 def test_lss_cell_index_and_pool_vs_golden(golden_dir):
     from heal_b200 import ops
-    g = torch.load(os.path.join(golden_dir, "lss_small.pt"), weights_only=False)
+    g = golden.load(os.path.join(golden_dir, "lss_small.pt"))
     cfg = g["cfg"]
     fr = lss.create_frustum(cfg["grid_conf"], cfg["data_aug_conf"]["final_dim"], cfg["img_downsample"])
     dx, bx, nx = lss.gen_dx_bx(cfg["grid_conf"]["xbound"], cfg["grid_conf"]["ybound"], cfg["grid_conf"]["zbound"])
@@ -75,7 +77,7 @@ def test_lss_pool_sorted_vs_golden_both_layouts_and_deterministic(golden_dir):
     """heal_lss_pool_sorted (cell-sorted interval sums, no atomics): equals the exact per-cell sum, the unmodified reference's
     cumsum output within its own rounding, for NCHW inputs and for the channels-last fused-heads layout, bit-identical run to run."""
     from heal_b200 import ops
-    g = torch.load(os.path.join(golden_dir, "lss_small.pt"), weights_only=False)
+    g = golden.load(os.path.join(golden_dir, "lss_small.pt"))
     cfg = g["cfg"]
     fr = lss.create_frustum(cfg["grid_conf"], cfg["data_aug_conf"]["final_dim"], cfg["img_downsample"])
     dx, bx, nx = lss.gen_dx_bx(cfg["grid_conf"]["xbound"], cfg["grid_conf"]["ybound"], cfg["grid_conf"]["zbound"])
@@ -104,7 +106,7 @@ def test_lss_pool_sorted_vs_golden_both_layouts_and_deterministic(golden_dir):
 
 
 def test_camera_trunk_on_the_conv_engine_vs_torch():
-    """CamEncode_Resnet101.heads_nhwc (space-to-depth stem on tcgen05, heal_maxpool3x3s2, Bottlenecks, fused heads) == the torch
+    """CamEncode_Resnet101.heads_nhwc (space-to-depth stem on wgmma, heal_maxpool3x3s2, Bottlenecks, fused heads) == the torch
     modules' own forward (torchvision resnet101 conv1..layer2 + 1x1 heads, lss_submodule.py:140-233) on CPU."""
     from heal_b200 import engine
     from heal_b200.models.heter_encoders import CamEncode_Resnet101

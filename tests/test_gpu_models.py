@@ -6,6 +6,8 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import golden
+
 from oracle import nets, procedural, make_golden, voxelizer
 
 pytestmark = pytest.mark.gpu
@@ -58,7 +60,7 @@ def _restore_precision():
 def test_heter_pyramid_collab_vs_reference_golden(golden_dir, prec, tol):
     from heal_b200 import engine
     engine.set_precision(prec)
-    g = torch.load(os.path.join(golden_dir, "heter_pyramid_collab_small.pt"), weights_only=False)
+    g = golden.load(os.path.join(golden_dir, "heter_pyramid_collab_small.pt"))
     model, _ = _build(g["args"], g["shapes"])
     data = _to_cuda(g["data"])
     data["record_len"] = g["data"]["record_len"]
@@ -80,7 +82,7 @@ def test_heter_pyramid_collab_gpu_voxelize_path_vs_oracle(prec, tol):
     rng_ = [-25.6, -25.6, -3, 25.6, 25.6, 1]      # 128 x 128 pillars, fusion at 64 x 64
     args["lidar_range"] = rng_
     args["m1"]["encoder_args"]["lidar_range"] = rng_
-    g = torch.load(os.path.join(os.path.dirname(__file__), "golden", "heter_pyramid_collab_small.pt"), weights_only=False)
+    g = golden.load(os.path.join(os.path.dirname(__file__), "golden", "heter_pyramid_collab_small.pt"))
     model, sd = _build(args, g["shapes"])
     sc = synth.scene(11, n_agents=3, rings=32, azimuth=512)
     per_agent = [voxelizer.points_to_voxel_c(p, [0.4, 0.4, 4], rng_, 32, 70000) for p in sc["points"]]
@@ -115,7 +117,7 @@ def test_agent_sharded_world1_equals_plain_forward():
     """forward_agent_sharded (pack -> gather -> unpack -> fuse tail) on one rank == the plain module forward."""
     from heal_b200 import synth, parallel
     args = make_golden.small_model_args()
-    g = torch.load(os.path.join(os.path.dirname(__file__), "golden", "heter_pyramid_collab_small.pt"), weights_only=False)
+    g = golden.load(os.path.join(os.path.dirname(__file__), "golden", "heter_pyramid_collab_small.pt"))
     model, _ = _build(args, g["shapes"])
     sc = synth.scene(5, n_agents=3, rings=16, azimuth=256)
     offs = np.concatenate([[0], np.cumsum([p.shape[0] for p in sc["points"]])]).astype(np.int32)
@@ -133,7 +135,7 @@ def test_agent_sharded_frame_world1_equals_plain_forward():
     captured graph) on one rank == the plain module forward, bit for bit."""
     from heal_b200 import synth, parallel
     args = make_golden.small_model_args()
-    g = torch.load(os.path.join(os.path.dirname(__file__), "golden", "heter_pyramid_collab_small.pt"), weights_only=False)
+    g = golden.load(os.path.join(os.path.dirname(__file__), "golden", "heter_pyramid_collab_small.pt"))
     model, _ = _build(args, g["shapes"])
     for n_agents in (3, 1):
         sc = synth.scene(5, n_agents=n_agents, rings=16, azimuth=256)
@@ -173,7 +175,7 @@ def test_frame_graph_and_pipeline_equal_eager():
     from heal_b200 import synth
     from heal_b200.graph import FrameGraph, FramePipeline
     args = make_golden.small_model_args()
-    g = torch.load(os.path.join(os.path.dirname(__file__), "golden", "heter_pyramid_collab_small.pt"), weights_only=False)
+    g = golden.load(os.path.join(os.path.dirname(__file__), "golden", "heter_pyramid_collab_small.pt"))
     model, _ = _build(args, g["shapes"])
     scenes = []
     for seed, az in ((3, 256), (4, 192), (5, 320), (6, 256), (7, 224)):

@@ -7,6 +7,8 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import golden
+
 from oracle import nets, procedural, make_golden, voxelizer, sparse_conv as sc, lss
 
 pytestmark = pytest.mark.gpu
@@ -48,7 +50,7 @@ def test_heter_model_baseline_att_vs_reference_golden(golden_dir, prec, tol):
     from heal_b200 import engine
     from heal_b200.models.heter_model_baseline import HeterModelBaseline
     engine.set_precision(prec)
-    g = torch.load(os.path.join(golden_dir, "heter_model_baseline_att_small.pt"), weights_only=False)
+    g = golden.load(os.path.join(golden_dir, "heter_model_baseline_att_small.pt"))
     m = HeterModelBaseline(copy.deepcopy(g["args"])).eval()
     m.load_state_dict(procedural.make_state_dict(g["shapes"]), strict=True)
     m = m.cuda()
@@ -137,7 +139,7 @@ def test_c4_lss_plus_pointpillar_hetero_vs_oracle(prec, tol):
     m = HeterPyramidCollab(copy.deepcopy(args)).eval()
     sd = procedural.make_state_dict(procedural.shapes_of(m))
     m.load_state_dict(sd, strict=True)
-    g = torch.load(os.path.join(os.path.dirname(__file__), "golden", "heter_pyramid_collab_small.pt"), weights_only=False)
+    g = golden.load(os.path.join(os.path.dirname(__file__), "golden", "heter_pyramid_collab_small.pt"))
     lidar = {k: v for k, v in g["data"]["inputs_m1"].items()}
     keep = lidar["voxel_coords"][:, 0] == 0                 # agent 0 is the lidar agent
     lidar = {k: v[keep] for k, v in lidar.items()}

@@ -9,6 +9,8 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import golden
+
 from oracle import make_golden
 from oracle import postprocess as opp
 
@@ -17,7 +19,7 @@ pytestmark = pytest.mark.gpu
 
 @pytest.fixture(scope="module")
 def gold(golden_dir):
-    return torch.load(os.path.join(golden_dir, "postprocess.pt"), weights_only=False)
+    return golden.load(os.path.join(golden_dir, "postprocess.pt"))
 
 
 def _run_gpu(params, anchors, cls, reg, dirp, T):

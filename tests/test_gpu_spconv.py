@@ -71,7 +71,7 @@ def test_strided_conv_vs_oracle(ksize, stride, pad, shape):
 
 @pytest.mark.parametrize("cin,cout,n", [(16, 16, 777), (16, 32, 5000), (32, 32, 3000), (32, 64, 4100), (64, 64, 2000), (64, 128, 1500)])
 def test_subm_conv_tensor_core_vs_oracle(cin, cout, n):
-    """heal_spconv_gather_gemm_tc (tcgen05, split-bf16 rows, cp.async gather) vs the oracle: fp32-equivalent (2^-16 per product)."""
+    """heal_spconv_gather_gemm_tc (wgmma, split-bf16 rows, cp.async gather) vs the oracle: fp32-equivalent (2^-16 per product)."""
     from heal_b200 import ops
     rng = np.random.default_rng(100 + cin + cout)
     shape, B = [21, 64, 64], 2

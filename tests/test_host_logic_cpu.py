@@ -6,6 +6,8 @@ import os
 import numpy as np
 import torch
 
+from oracle import golden
+
 from oracle import make_golden
 
 
@@ -38,13 +40,13 @@ def test_state_dict_keys_match_reference(golden_dir):
     """The goldens record the UNMODIFIED reference models' {key: shape} tables; the mirrors must reproduce them exactly."""
     from heal_b200.models.heter_pyramid_collab import HeterPyramidCollab
     from heal_b200.models.heter_model_baseline import HeterModelBaseline
-    g = torch.load(os.path.join(golden_dir, "heter_pyramid_collab_small.pt"), weights_only=False)
+    g = golden.load(os.path.join(golden_dir, "heter_pyramid_collab_small.pt"))
     m = HeterPyramidCollab(copy.deepcopy(g["args"]))
     assert {k: tuple(v.shape) for k, v in m.state_dict().items()} == {k: tuple(v) for k, v in g["shapes"].items()}
-    g = torch.load(os.path.join(golden_dir, "heter_model_baseline_att_small.pt"), weights_only=False)
+    g = golden.load(os.path.join(golden_dir, "heter_model_baseline_att_small.pt"))
     m = HeterModelBaseline(copy.deepcopy(g["args"]))
     assert {k: tuple(v.shape) for k, v in m.state_dict().items()} == {k: tuple(v) for k, v in g["shapes"].items()}
-    g = torch.load(os.path.join(golden_dir, "base_bev_backbone_small.pt"), weights_only=False)
+    g = golden.load(os.path.join(golden_dir, "base_bev_backbone_small.pt"))
     from heal_b200.models.sub_modules.base_bev_backbone import BaseBEVBackbone
     m = BaseBEVBackbone(copy.deepcopy(g["cfg"]), 64)
     assert {k: tuple(v.shape) for k, v in m.state_dict().items()} == {k: tuple(v) for k, v in g["shapes"].items()}
@@ -87,7 +89,7 @@ def test_postprocessor_anchor_box_equals_reference_golden(golden_dir):
     import numpy as np
     import torch
     from heal_b200.data_utils.post_processor import build_postprocessor
-    g = torch.load(os.path.join(golden_dir, "postprocess.pt"), weights_only=False)
+    g = golden.load(os.path.join(golden_dir, "postprocess.pt"))
     pp = build_postprocessor(copy.deepcopy(g["params"]), train=False)
     a = pp.generate_anchor_box()
     assert a.dtype == np.float64 and np.array_equal(a, g["anchors"].numpy())

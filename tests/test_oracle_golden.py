@@ -6,11 +6,13 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import golden
+
 from oracle import nets, procedural
 
 
 def _load(golden_dir, name):
-    return torch.load(os.path.join(golden_dir, name), weights_only=False)
+    return golden.load(os.path.join(golden_dir, name))
 
 
 def test_heter_pyramid_collab_small(golden_dir):
@@ -85,7 +87,7 @@ def test_heter_model_baseline_att_small(golden_dir):
 def test_convnext_aligner_oracle_vs_reference_golden(golden_dir):
     """oracle.nets.convnext_aligner == the UNMODIFIED reference AlignNet(convnext) output (feature_alignnet_modules.py:299-360)."""
     import os
-    g = torch.load(os.path.join(golden_dir, "convnext_aligner.pt"), weights_only=False)
+    g = golden.load(os.path.join(golden_dir, "convnext_aligner.pt"))
     sd = {"al." + k: v for k, v in procedural.make_state_dict(g["shapes"]).items()}
     with torch.no_grad():
         y = nets.convnext_aligner(g["x"], sd, "al", g["cfg"]["args"]["num_of_blocks"])

@@ -6,12 +6,14 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import golden
+
 from oracle import postprocess as opp
 
 
 @pytest.fixture(scope="module")
 def gold(golden_dir):
-    return torch.load(os.path.join(golden_dir, "postprocess.pt"), weights_only=False)
+    return golden.load(os.path.join(golden_dir, "postprocess.pt"))
 
 
 def test_anchor_box_matches_reference(gold):
