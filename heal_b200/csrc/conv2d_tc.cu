@@ -19,9 +19,9 @@
 //
 // Roles (384 threads): warpgroup 0 = TMA producer (warp 0 loops as a converged warp and issues under elect.sync; its
 // registers are handed to the consumers with setmaxnreg), warpgroups 1 and 2 = consumers: each runs the M = 64 wgmma of one
-// half of the 128-pixel tile, then both drain the tile together: accumulator chunk -> fp32 scratch in shared memory (rows
-// transposed from the wgmma fragment to one pixel per thread) -> bias / residual / ReLU -> hi/lo split -> swizzled smem
-// staging -> one cp.async.bulk.tensor store per 64-channel chunk (fp32 / transposed-conv outputs use direct stores).
+// half of the 128-pixel tile, then applies bias / residual / ReLU / hi-lo split to its accumulator fragment in place and
+// writes it to the fragment's positions of a swizzled smem staging tile -> one cp.async.bulk.tensor store per 64-channel
+// chunk (fp32 / transposed-conv / narrow outputs are stored from the fragment straight to global memory).
 // The producer keeps STAGES k-blocks in flight, so the next tile's operands arrive while the consumers run the epilogue.
 // Modes: stride 2 through TMA element strides; grouped 3x3 as 16-channel sub-block MMAs on block-diagonal 64-channel
 // tiles; "halo" (3x3, stride 1, one-row tiles, N = 64): one activation box of TW+2 pixels per kernel ROW, the three
@@ -75,7 +75,9 @@ struct TcP {
 // full coalesced line and the drain is asynchronous).
 // GELU: the exact-erf GELU epilogue (ConvNeXt pwconv1) lives in its OWN instantiations: this kernel is sensitive to code size
 // (an erff call inside every instantiation's epilogue cost the ReLU paths ~4 % of the C2 frame, A/B on the bench)
-template <int BLOCK_N, int STAGES, int STG, bool GELU = false>
+// GROUPED (p.blockdiag): the grouped conv's MMA shapes are their own instantiations too, so that each one issues a single
+// set of wgmma shapes on its accumulator registers (mixed shapes on the same registers make ptxas serialise the chain).
+template <int BLOCK_N, int STAGES, int STG, bool GELU = false, bool GROUPED = false>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
             const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR, const TcP p) {
@@ -96,9 +98,7 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     const int stage_bytes = p.halo ? (halo_a_bytes + p.wplanes * 3 * B_TILE_BYTES) : (p.planes * A_TILE_BYTES + p.wplanes * B_TILE_BYTES);
     const int stg_bytes = p.planes * A_TILE_BYTES;                        // one staging buffer: [plane][128 rows][128 B]
     uint8_t* stg = smem + (size_t)STAGES * stage_bytes;                   // 1024-aligned (stage_bytes is a multiple of 1024)
-    constexpr int SW = BLOCK_N < 64 ? BLOCK_N : 64;                       // accumulator columns per pass through the scratch
-    const uint32_t scr = smem_u32(stg + (size_t)STG * stg_bytes);         // fp32 scratch [128 rows][SW]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(stg + (size_t)STG * stg_bytes + BLOCK_M * SW * 4);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(stg + (size_t)STG * stg_bytes);
     // bars: full[STAGES], empty[STAGES], residual_full[3]
     const uint32_t bar_res = smem_u32(bars + 2 * STAGES);
     const uint32_t smem_base = smem_u32(smem);
@@ -107,8 +107,8 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // Split-bf16 products a_hi*b_hi + a_hi*b_lo + a_lo*b_hi.  For BLOCK_N <= 64 the hi and lo weight planes sit next to each other
     // in shared memory, so ONE MMA with N' = 2N computes a_hi x [b_hi | b_lo] (main | aux accumulator columns) and a second
-    // N-wide MMA adds a_lo x b_hi: 2 tensor-core instructions and 2 reads of the A slice per K step instead of 3.  The
-    // consumers add aux to main before the epilogue.  BLOCK_N = 128 keeps 3 MMAs (N' = 256 would need 128 accumulator
+    // N-wide MMA computes a_lo x b_hi into registers of its own: 2 tensor-core instructions and 2 reads of the A slice per K
+    // step instead of 3.  The consumers fold main + (aux + a_lo x b_hi) before the epilogue.  BLOCK_N = 128 keeps 3 MMAs (N' = 256 would need 128 accumulator
     // registers per thread).
     constexpr bool NCAT = (BLOCK_N <= 64);
     constexpr int NACC = NCAT ? 2 * BLOCK_N : BLOCK_N;            // accumulator columns per tile half
@@ -178,11 +178,12 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     } else {
         // ============================== consumers (warpgroups 1 and 2): wgmma, then the epilogue ==
         regs_inc<232>();
-        const int wg = (warp >> 2) - 1;                 // MMAs: tile rows [64 wg, 64 wg + 64)
-        const int quarter = warp & 3;
-        const int chalf = (warp - 4) >> 2;              // epilogue: which half of the tile's column chunks this warp drains
-        const int row = quarter * 32 + lane;            // epilogue: accumulator row = pixel within the tile
-        constexpr int CHUNK = (BLOCK_N >= 32) ? 32 : 16;
+        const int wg = (warp >> 2) - 1;                 // tile rows [64 wg, 64 wg + 64)
+        // This thread's part of the accumulator fragment (tc_prims.cuh): rows frow and frow + 8 of the tile, columns 8 j + fcol
+        // and 8 j + fcol + 1 of every 8-column group j, in d[4 j .. 4 j + 3].  Both rows have the same 128B-swizzle phase fswz.
+        const int ft = threadIdx.x & 127;
+        const int frow = 64 * wg + 16 * (ft >> 5) + ((ft & 31) >> 2), fcol = 2 * (ft & 3);
+        const int fswz = (ft >> 2) & 7;
         int stg_count = 0;
         const bool split = (p.planes == 2);                      // activations carry a lo plane
         const bool wsplit = (p.wplanes == 2);                    // weights carry a lo plane
@@ -191,10 +192,15 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         const int ntap = p.halo ? 3 : 1;
         int stage = 0; uint32_t phase = 0;
         float d[NACC / 2];
+        float e[NCAT ? BLOCK_N / 2 : 1];                        // NCAT: a_lo*b_hi, or a_hi*b_hi with one weight plane
 #pragma unroll
         for (int i = 0; i < NACC / 2; ++i) d[i] = 0.f;
+#pragma unroll
+        for (int i = 0; i < (NCAT ? BLOCK_N / 2 : 1); ++i) e[i] = 0.f;
         // All k-blocks of one tile into d (this warpgroup's 64 rows); afterwards d[0, BLOCK_N / 2) is the fragment of the
-        // BLOCK_N logical columns (main + aux folded).
+        // BLOCK_N logical columns (main + (aux + a_lo*b_hi)).  With NCAT every MMA shape has a register array of its own (the
+        // N = BLOCK_N ones write e, not the first half of d): in-flight MMAs of different N on overlapping registers make ptxas
+        // serialise the whole wgmma chain.
         auto mma_tile = [&]() {
             int prev = -1;
             for (int kb = 0; kb < kblocks; ++kb) {
@@ -210,30 +216,31 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 #pragma unroll
                     for (int k = 0; k < BLOCK_K / 16; ++k) {
                         const uint64_t a_hi = gmma_desc_sw128_off(ah + k * 32, p.bo_mode), a_lo = gmma_desc_sw128_off(al + k * 32, p.bo_mode);
-                        if (p.blockdiag) {
+                        if constexpr (GROUPED) {
                             if constexpr (BLOCK_N == 64) {
                                 // Grouped conv: channels-per-group divides 16, so output channels [16k,16k+16) of this 64-block depend
                                 // only on input channels [16k,16k+16): one M64 x N16 x K16 product per 16-channel sub-block, into
-                                // its own accumulator registers d[16k ..] ([main16 | aux16]) or d[8k ..].
+                                // its own accumulator registers d[16k ..] ([main16 | aux16]) and e[8k ..], or d[8k ..].
                                 // sub-block k: [plane][16 rows] of 128 B rows at K offset k*16 elements, or packed 32 B rows
                                 const uint32_t bk = p.bdiag ? bs + k * p.wplanes * 512 : bs + k * sub_bytes + k * 32;
                                 const uint64_t bd = p.bdiag ? gmma_desc_sw32(bk) : gmma_desc_sw128(bk);
                                 const uint32_t f0 = (kb == 0 && s == 0) ? 0u : 1u;
                                 if (wsplit) {
                                     wgmma_bf16<32>(d + 16 * k, a_hi, bd, f0);               // [a_hi*b_hi | a_hi*b_lo]
-                                    if (split) wgmma_bf16<16>(d + 16 * k, a_lo, bd, 1u);    // += a_lo*b_hi
+                                    if (split) wgmma_bf16<16>(e + 8 * k, a_lo, bd, f0);     // a_lo*b_hi
                                 } else {
-                                    wgmma_bf16<16>(d + 8 * k, a_hi, bd, f0);
+                                    wgmma_bf16<16>(e + 8 * k, a_hi, bd, f0);
                                 }
                             }
                         } else {
                             const uint32_t first = (kb == 0 && s == 0 && k == 0) ? 0u : 1u;
                             const uint64_t b_hi = gmma_desc_sw128(bs + k * 32);
                             if (!wsplit) {
-                                wgmma_bf16<BLOCK_N>(d, a_hi, b_hi, first);
+                                if constexpr (NCAT) wgmma_bf16<BLOCK_N>(e, a_hi, b_hi, first);
+                                else wgmma_bf16<BLOCK_N>(d, a_hi, b_hi, first);
                             } else if constexpr (NCAT) {
                                 wgmma_bf16<2 * BLOCK_N>(d, a_hi, b_hi, first);               // [a_hi*b_hi | a_hi*b_lo]
-                                if (split) wgmma_bf16<BLOCK_N>(d, a_lo, b_hi, 1u);           // += a_lo*b_hi
+                                if (split) wgmma_bf16<BLOCK_N>(e, a_lo, b_hi, first);        // a_lo*b_hi
                             } else {
                                 const uint64_t b_lo = gmma_desc_sw128(bs + B_TILE_BYTES + k * 32);
                                 wgmma_bf16<BLOCK_N>(d, a_hi, b_lo, first);
@@ -252,62 +259,26 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             wgmma_wait<0>();
             if (prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev);
             if constexpr (NCAT) {
-                if (wsplit) {
-                    if constexpr (BLOCK_N == 64) {
-                        if (p.blockdiag) {
+                if (!wsplit) {
 #pragma unroll
-                            for (int k = 0; k < 4; ++k)
+                    for (int i = 0; i < BLOCK_N / 2; ++i) d[i] = e[i];
+                } else if constexpr (GROUPED && BLOCK_N == 64) {   // the same fold as k_gconv3x3_ring (the two kernels agree bit for bit)
 #pragma unroll
-                                for (int q = 0; q < 8; ++q) d[8 * k + q] = d[16 * k + q] + d[16 * k + 8 + q];
-                            return;
-                        }
-                    }
+                    for (int k = 0; k < 4; ++k)
 #pragma unroll
-                    for (int i = 0; i < BLOCK_N / 2; ++i) d[i] += d[i + BLOCK_N / 2];
+                        for (int q = 0; q < 8; ++q)
+                            d[8 * k + q] = d[16 * k + q] + (split ? d[16 * k + 8 + q] + e[8 * k + q] : d[16 * k + 8 + q]);
+                } else {
+#pragma unroll
+                    for (int i = 0; i < BLOCK_N / 2; ++i) d[i] += split ? d[i + BLOCK_N / 2] + e[i] : d[i + BLOCK_N / 2];
                 }
             }
         };
-        // logical accumulator columns [c0, c0 + SW) of the whole tile -> scratch (both warpgroups), readable after the barrier
-        auto to_scratch = [&](int c0) {
-            epi_bar(3);
-            frag_to_scratch<BLOCK_N / 2, SW>(d, scr, 64 * wg, c0);
-            epi_bar(3);
-        };
-        // N logical columns [col0, col0 + N) of this thread's row, from the scratch chunk that holds them -> raw (fp32 bits)
-        auto ld_acc = [&](int col0, uint32_t* raw) {
-            scratch_row<SW, (BLOCK_N >= 32 ? 32 : 16)>(scr, row, col0 % SW, raw);
-        };
-        // Residual prefetch (TMA-store epilogue, split/bf16 residual): the 2 x 4 x 16 B of this thread's row for the NEXT 64-channel
-        // chunk are requested one chunk ahead, so their DRAM latency hides behind the current chunk (and the wait for the MMAs)
-        // instead of stalling every 8-channel group.
-        uint4 rn_h[4], rn_l[4];
         // compiled only into the instantiations with at least two staging buffers (the ones dispatched with a residual)
         constexpr bool RES_TMA_OK = (STG >= 2);
         const bool res_tma = RES_TMA_OK && p.res_tma && !(p.dbg & 8);
-        constexpr bool RES_PF = (STG == 1 && BLOCK_N == 64);      // the halo configuration: no room for 3 staging buffers
-        const bool res_pf = RES_PF && p.tma_out && p.res_split && !(p.dbg & 8);
-        auto res_fetch = [&](int tile_, int c64_) {
-            const int nt_ = tile_ % p.n_tiles, mt_ = tile_ / p.n_tiles;
-            const int tw_ = mt_ % p.tiles_w; const int t2_ = mt_ / p.tiles_w;
-            const int th_ = t2_ % p.tiles_h; const int img_ = t2_ / p.tiles_h;
-            const int oh_ = th_ * p.TH + row / p.TW, ow_ = tw_ * p.TW + row % p.TW;
-            const int ng_ = nt_ * BLOCK_N;
-            const int q_ = ng_ / p.coutp, c0_ = ng_ % p.coutp + c64_ * 64 + chalf * 32;
-            const size_t pix_ = ((size_t)img_ * (p.Ho * p.up) + (size_t)(oh_ * p.up + q_ / p.up)) * (size_t)(p.Wo * p.up) + (size_t)(ow_ * p.up + q_ % p.up);
-            const bool ok_ = (oh_ < p.Ho) && (ow_ < p.Wo);
-            const __nv_bfloat16* rp = p.res_split + pix_ * p.res_cs + p.res_co + c0_;
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-                rn_h[g] = make_uint4(0u, 0u, 0u, 0u); rn_l[g] = make_uint4(0u, 0u, 0u, 0u);
-                if (ok_ && c0_ + g * 8 + 8 <= p.Cout) {
-                    rn_h[g] = __ldg(reinterpret_cast<const uint4*>(rp + g * 8));
-                    if (p.planes == 2) rn_l[g] = __ldg(reinterpret_cast<const uint4*>(rp + p.res_plane + g * 8));
-                }
-            }
-        };
-        if (RES_PF && res_pf && (int)blockIdx.x < total_tiles) res_fetch(blockIdx.x, 0);
-        // TMA variant (STG == 3): residual chunk i+1 lands in staging buffer (i+1) % 3 while chunk i is processed; the epilogue
-        // then adds it IN PLACE (same swizzled 16 B slots it will overwrite with the output) -- fully coalesced, no registers.
+        // residual chunk i+1 lands in staging buffer (i+1) % STG while chunk i is processed; the epilogue then adds it IN PLACE
+        // (the fragment's own swizzled slots, which it overwrites with the output) -- fully coalesced, no global loads per thread.
         auto res_tma_issue = [&](int tile_, int c64_, int buf_) {
             const int nt_ = tile_ % p.n_tiles, mt_ = tile_ / p.n_tiles;
             const int tw_ = mt_ % p.tiles_w; const int t2_ = mt_ / p.tiles_w;
@@ -320,20 +291,30 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             const int nt = tile % p.n_tiles, mt = tile / p.n_tiles;
             const int tw_i = mt % p.tiles_w; const int t2 = mt / p.tiles_w;
             const int th_i = t2 % p.tiles_h; const int img = t2 / p.tiles_h;
-            const int oh = th_i * p.TH + row / p.TW, ow = tw_i * p.TW + row % p.TW;
-            const bool valid = (oh < p.Ho) && (ow < p.Wo);
             const int n_glob = nt * BLOCK_N;
             const int q = n_glob / p.coutp, ch0 = n_glob % p.coutp;   // q = sub-position of a transposed conv (0 otherwise)
             const int ui = q / p.up, uj = q % p.up;
-            const size_t pix = ((size_t)img * (p.Ho * p.up) + (size_t)(oh * p.up + ui)) * (size_t)(p.Wo * p.up) + (size_t)(ow * p.up + uj);
+            // the fragment's two rows: in range, and the output pixel's linear index
+            bool valid[2]; size_t pix[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = frow + 8 * h;
+                const int oh = th_i * p.TH + r / p.TW, ow = tw_i * p.TW + r % p.TW;
+                valid[h] = (oh < p.Ho) && (ow < p.Wo);
+                pix[h] = ((size_t)img * (p.Ho * p.up) + (size_t)(oh * p.up + ui)) * (size_t)(p.Wo * p.up) + (size_t)(ow * p.up + uj);
+            }
             mma_tile();
             if constexpr (STG > 0 && BLOCK_N >= 64) {
               if (p.tma_out) {
                 const uint32_t stg_base = smem_u32(stg);
-#pragma unroll 1
+#pragma unroll
                 for (int c64 = 0; c64 < BLOCK_N / 64; ++c64) {
-                    to_scratch(c64 * 64);
                     const int b = stg_count % STG;
+                    // the chunk's bias pairs, requested before the waits (the shared-memory stores below are compiler barriers)
+                    float2 bb[8];
+#pragma unroll
+                    for (int jj = 0; jj < 8; ++jj)
+                        bb[jj] = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + ch0 + 64 * c64 + 8 * jj + fcol)) : make_float2(0.f, 0.f);
                     if (res_tma) {
                         // (A') the store that last used buffer (i+1) % STG has been read out -> request residual(i+1) into it, then wait
                         // for residual(i) in buffer b (STG == 3: a full chunk of lead; STG == 2: the lead is the chunk minus the store drain)
@@ -349,81 +330,47 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                         if (warp == 4 && lane == 0) bulk_wait_read<STG - 1>();
                         epi_bar(1);
                     }
-                    // (B) this warp's 32 columns of the 64-column chunk -> registers -> epilogue -> swizzled smem.  Loads first (bias:
-                    // warp-uniform 16 B broadcasts; residual: this thread's eight 16 B slots of the staging buffer), then the
-                    // arithmetic, then the eight 16 B stores back to back.
-                    uint32_t raw[32];
-                    const int col0 = c64 * 64 + chalf * 32;
-                    float bv[32];
+                    // (B) this thread's 2 rows x 16 columns of the 64-column chunk, straight from the fragment: bias, residual (read
+                    // from the staging buffer at the fragment's swizzled slots), activation, hi/lo split, written back to the same
+                    // slots (bank-conflict free: the 8 rows of a warp have 8 different swizzle phases).
+                    const uint32_t row0 = stg_base + b * stg_bytes + frow * 128 + 2 * fcol;   // row frow + 8 is 1024 B further
 #pragma unroll
-                    for (int g = 0; g < 8; ++g) {
-                        float4 t = p.bias ? __ldg(reinterpret_cast<const float4*>(p.bias + ch0 + col0) + g) : make_float4(0.f, 0.f, 0.f, 0.f);
-                        bv[4 * g] = t.x; bv[4 * g + 1] = t.y; bv[4 * g + 2] = t.z; bv[4 * g + 3] = t.w;
-                    }
-                    const uint32_t srow = stg_base + b * stg_bytes + row * 128;
-                    uint4 rh[4], rl[4];
+                    for (int jj = 0; jj < 8; ++jj) {
+                        const int j = c64 * 8 + jj;
+                        const int c = ch0 + 8 * j + fcol;
+                        const uint32_t a0 = row0 + (uint32_t)((jj ^ fswz) << 4);
+                        float v[4] = {d[4 * j] + bb[jj].x, d[4 * j + 1] + bb[jj].y, d[4 * j + 2] + bb[jj].x, d[4 * j + 3] + bb[jj].y};
+                        if (res_tma) {
+                            // residual pairs [hi row0, hi row0 + 8, lo row0, lo row0 + 8]
+                            const uint32_t rs[4] = {lds_b32(a0), lds_b32(a0 + 1024), split ? lds_b32(a0 + A_TILE_BYTES) : 0u,
+                                                    split ? lds_b32(a0 + A_TILE_BYTES + 1024) : 0u};
 #pragma unroll
-                    for (int g8 = 0; g8 < 4; ++g8) { rh[g8] = make_uint4(0u, 0u, 0u, 0u); rl[g8] = make_uint4(0u, 0u, 0u, 0u); }
-                    bool have_res = false;
-                    if (res_tma) {
-                        have_res = true;
+                            for (int h = 0; h < 2; ++h) { v[2 * h] += bf16_lo_f(rs[h]); v[2 * h + 1] += bf16_hi_f(rs[h]); }
+                            if (split) {
 #pragma unroll
-                        for (int g8 = 0; g8 < 4; ++g8) {
-                            const uint32_t chunk16 = (uint32_t)(((chalf * 4 + g8) ^ (row & 7)) * 16);      // 128B swizzle
-                            asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(rh[g8].x), "=r"(rh[g8].y), "=r"(rh[g8].z), "=r"(rh[g8].w) : "r"(srow + chunk16));
-                            if (p.planes == 2)
-                                asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(rl[g8].x), "=r"(rl[g8].y), "=r"(rl[g8].z), "=r"(rl[g8].w) : "r"(srow + A_TILE_BYTES + chunk16));
-                        }
-                    } else if (RES_PF && res_pf) {
-                        have_res = true;        // register-prefetched one chunk ago (rn_h / rn_l)
-                    }
-                    const uint4* res_h = RES_PF ? rn_h : rh;
-                    const uint4* res_l = RES_PF ? rn_l : rl;
-                    ld_acc(col0, raw);
-                    uint32_t hw[4][4], lw[4][4];
-#pragma unroll
-                    for (int g8 = 0; g8 < 4; ++g8) {
-                        const int c = ch0 + col0 + g8 * 8;
-                        float v[8];
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) v[j] = __uint_as_float(raw[g8 * 8 + j]) + bv[g8 * 8 + j];
-                        if (have_res) {
-                            const __nv_bfloat16* hb = reinterpret_cast<const __nv_bfloat16*>(&res_h[g8]);
-                            const __nv_bfloat16* lb = reinterpret_cast<const __nv_bfloat16*>(&res_l[g8]);
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) v[j] += __bfloat162float(hb[j]);
-                            if (p.planes == 2) {
-#pragma unroll
-                                for (int j = 0; j < 8; ++j) v[j] += __bfloat162float(lb[j]);
+                                for (int h = 0; h < 2; ++h) { v[2 * h] += bf16_lo_f(rs[2 + h]); v[2 * h + 1] += bf16_hi_f(rs[2 + h]); }
                             }
-                        } else if (valid && p.res_f32 && !(p.dbg & 8)) {
-                            const float* rp = p.res_f32 + pix * p.res_cs + p.res_co + c;
+                        } else if (p.res_f32 && !(p.dbg & 8)) {
 #pragma unroll
-                            for (int j = 0; j < 8; ++j) v[j] += __ldg(rp + j);
+                            for (int h = 0; h < 2; ++h) {
+                                if (valid[h]) {
+                                    const float* rp = p.res_f32 + pix[h] * p.res_cs + p.res_co + c;
+                                    v[2 * h] += __ldg(rp); v[2 * h + 1] += __ldg(rp + 1);
+                                }
+                            }
                         }
                         if constexpr (GELU) {
 #pragma unroll
-                            for (int j = 0; j < 8; ++j) v[j] = heal_act_fn(v[j], 2);
+                            for (int i = 0; i < 4; ++i) v[i] = heal_act_fn(v[i], 2);
                         } else if (p.relu) {
 #pragma unroll
-                            for (int j = 0; j < 8; ++j) v[j] = fmaxf(v[j], 0.f);
+                            for (int i = 0; i < 4; ++i) v[i] = fmaxf(v[i], 0.f);
                         }
-                        float lo[8];
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) lo[j] = v[j] - __bfloat162float(__float2bfloat16_rn(v[j]));
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) { hw[g8][j] = pack_bf16(v[2 * j], v[2 * j + 1]); lw[g8][j] = pack_bf16(lo[2 * j], lo[2 * j + 1]); }
-                    }
-                    if (RES_PF && res_pf) {      // registers consumed: request the next chunk's residual
-                        if (c64 + 1 < BLOCK_N / 64) res_fetch(tile, c64 + 1);
-                        else if (tile + (int)gridDim.x < total_tiles) res_fetch(tile + gridDim.x, 0);
-                    }
-#pragma unroll
-                    for (int g8 = 0; g8 < 4; ++g8) {
-                        const uint32_t chunk16 = (uint32_t)(((chalf * 4 + g8) ^ (row & 7)) * 16);      // 128B swizzle
-                        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(srow + chunk16), "r"(hw[g8][0]), "r"(hw[g8][1]), "r"(hw[g8][2]), "r"(hw[g8][3]) : "memory");
-                        if (p.planes == 2)
-                            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(srow + A_TILE_BYTES + chunk16), "r"(lw[g8][0]), "r"(lw[g8][1]), "r"(lw[g8][2]), "r"(lw[g8][3]) : "memory");
+                        sts_b32(a0, pack_bf16(v[0], v[1])); sts_b32(a0 + 1024, pack_bf16(v[2], v[3]));
+                        if (split) {
+                            sts_b32(a0 + A_TILE_BYTES, pack_bf16(bf16_rest(v[0]), bf16_rest(v[1])));
+                            sts_b32(a0 + A_TILE_BYTES + 1024, pack_bf16(bf16_rest(v[2]), bf16_rest(v[3])));
+                        }
                     }
                     fence_async_smem();
                     epi_bar(2);
@@ -437,82 +384,57 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                 continue;
               }
             }
-#pragma unroll 1
-            for (int c0 = 0; c0 < BLOCK_N; c0 += SW) {
-                to_scratch(c0);
-                if (chalf >= SW / CHUNK) continue;
-                const int cc = c0 / CHUNK + chalf;
-                uint32_t raw[CHUNK];
-                ld_acc(cc * CHUNK, raw);
-                const int c_first = ch0 + cc * CHUNK;
-                if (valid && c_first < p.Cout) {
+            // direct stores (fp32 outputs, transposed convs, N = 16 / 32, Cout % 64 != 0): each thread writes its fragment's
+            // column pairs of its two rows
 #pragma unroll
-                    for (int g8 = 0; g8 < CHUNK / 8; ++g8) {
-                        const int c = c_first + g8 * 8;
-                        if (c >= p.Cout) break;
-                        float v[8];
+            for (int j = 0; j < BLOCK_N / 8; ++j) {
+                const int c = ch0 + 8 * j + fcol;
+                if (c >= p.Cout) continue;
+                const bool two = c + 1 < p.Cout;
+                const float b0 = p.bias ? __ldg(p.bias + c) : 0.f, b1 = (two && p.bias) ? __ldg(p.bias + c + 1) : 0.f;
 #pragma unroll
-                        for (int j = 0; j < 8; ++j) v[j] = __uint_as_float(raw[g8 * 8 + j]) + ((c + j < p.Cout && p.bias) ? __ldg(p.bias + c + j) : 0.f);
-                        const bool full8 = (c + 8 <= p.Cout);
-                        if (p.res_split) {
-                            const __nv_bfloat16* rp = p.res_split + pix * p.res_cs + p.res_co + c;
-                            if (full8 && (((p.res_cs | p.res_co) & 7) == 0)) {
-                                uint4 h = __ldg(reinterpret_cast<const uint4*>(rp));
-                                const __nv_bfloat16* hb = reinterpret_cast<const __nv_bfloat16*>(&h);
-#pragma unroll
-                                for (int j = 0; j < 8; ++j) v[j] += __bfloat162float(hb[j]);
-                                if (p.planes == 2) {
-                                    uint4 l = __ldg(reinterpret_cast<const uint4*>(rp + p.res_plane));
-                                    const __nv_bfloat16* lb = reinterpret_cast<const __nv_bfloat16*>(&l);
-#pragma unroll
-                                    for (int j = 0; j < 8; ++j) v[j] += __bfloat162float(lb[j]);
-                                }
-                            } else {
-                                for (int j = 0; j < 8 && c + j < p.Cout; ++j) {
-                                    v[j] += __bfloat162float(rp[j]);
-                                    if (p.planes == 2) v[j] += __bfloat162float(rp[p.res_plane + j]);
-                                }
-                            }
-                        } else if (p.res_f32) {
-                            const float* rp = p.res_f32 + pix * p.res_cs + p.res_co + c;
-                            for (int j = 0; j < 8 && c + j < p.Cout; ++j) v[j] += __ldg(rp + j);
+                for (int h = 0; h < 2; ++h) {
+                    if (!valid[h]) continue;
+                    float v0 = d[4 * j + 2 * h] + b0, v1 = d[4 * j + 2 * h + 1] + b1;
+                    if (p.res_split) {
+                        const __nv_bfloat16* rp = p.res_split + pix[h] * p.res_cs + p.res_co + c;
+                        v0 += __bfloat162float(rp[0]);
+                        if (two) v1 += __bfloat162float(rp[1]);
+                        if (split) {
+                            v0 += __bfloat162float(rp[p.res_plane]);
+                            if (two) v1 += __bfloat162float(rp[p.res_plane + 1]);
                         }
-                        if constexpr (GELU) {
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) v[j] = heal_act_fn(v[j], 2);
-                        } else if (p.relu) {
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) v[j] = fmaxf(v[j], 0.f);
-                        }
-                        if (p.out_split && !((p.dbg & 1) && v[0] != 1.2345e30f)) {
-                            __nv_bfloat16* op = p.out_split + pix * p.out_cs + p.out_co + c;
-                            float lo[8];
-                            uint32_t hw[4], lw[4];
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                float h = __bfloat162float(__float2bfloat16_rn(v[j]));
-                                lo[j] = v[j] - h;
-                            }
-#pragma unroll
-                            for (int j = 0; j < 4; ++j) { hw[j] = pack_bf16(v[2 * j], v[2 * j + 1]); lw[j] = pack_bf16(lo[2 * j], lo[2 * j + 1]); }
-                            if (full8 && (((p.out_cs | p.out_co) & 7) == 0)) {
-                                *reinterpret_cast<uint4*>(op) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                                if (p.planes == 2) *reinterpret_cast<uint4*>(op + p.out_plane) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-                            } else {
-                                for (int j = 0; j < 8 && c + j < p.Cout; ++j) {
-                                    op[j] = __float2bfloat16_rn(v[j]);
-                                    if (p.planes == 2) op[p.out_plane + j] = __float2bfloat16_rn(lo[j]);
-                                }
+                    } else if (p.res_f32) {
+                        const float* rp = p.res_f32 + pix[h] * p.res_cs + p.res_co + c;
+                        v0 += __ldg(rp);
+                        if (two) v1 += __ldg(rp + 1);
+                    }
+                    if constexpr (GELU) {
+                        v0 = heal_act_fn(v0, 2); v1 = heal_act_fn(v1, 2);
+                    } else if (p.relu) {
+                        v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f);
+                    }
+                    if (p.out_split && !((p.dbg & 1) && v0 != 1.2345e30f)) {
+                        __nv_bfloat16* op = p.out_split + pix[h] * p.out_cs + p.out_co + c;
+                        if (two && !((p.out_cs | p.out_co | p.out_plane) & 1)) {
+                            *reinterpret_cast<uint32_t*>(op) = pack_bf16(v0, v1);
+                            if (split) *reinterpret_cast<uint32_t*>(op + p.out_plane) = pack_bf16(bf16_rest(v0), bf16_rest(v1));
+                        } else {
+                            op[0] = __float2bfloat16_rn(v0);
+                            if (split) op[p.out_plane] = __float2bfloat16_rn(bf16_rest(v0));
+                            if (two) {
+                                op[1] = __float2bfloat16_rn(v1);
+                                if (split) op[p.out_plane + 1] = __float2bfloat16_rn(bf16_rest(v1));
                             }
                         }
-                        if (p.out_f32 && !((p.dbg & 1) && v[0] != 1.2345e30f)) {
-                            float* op = p.out_f32 + pix * p.out32_cs + p.out32_co + c;
-                            if (full8 && (((p.out32_cs | p.out32_co) & 3) == 0)) {
-                                stg_f4(op, make_float4(v[0], v[1], v[2], v[3]));
-                                stg_f4(op + 4, make_float4(v[4], v[5], v[6], v[7]));
-                            } else {
-                                for (int j = 0; j < 8 && c + j < p.Cout; ++j) op[j] = v[j];
-                            }
+                    }
+                    if (p.out_f32 && !((p.dbg & 1) && v0 != 1.2345e30f)) {
+                        float* op = p.out_f32 + pix[h] * p.out32_cs + p.out32_co + c;
+                        if (two && !((p.out32_cs | p.out32_co) & 1)) {
+                            *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
+                        } else {
+                            op[0] = v0;
+                            if (two) op[1] = v1;
                         }
                     }
                 }
@@ -525,27 +447,28 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 
 // HEAL_TC_* measurement hooks (profiles/tc_experiment.py), read once per process instead of six getenv calls per launch.
 struct TcEnv {
-    int dbg, pdl, halo, bo, tma_store, res_tma, ring, deep, l2promo;
+    int dbg, pdl, halo, bo, tma_store, res_tma, ring, l2promo;
     TcEnv() {
         auto geti = [](const char* n, int dflt) { const char* e = getenv(n); return e ? atoi(e) : dflt; };
         dbg = geti("HEAL_TC_DBG", 0); pdl = geti("HEAL_TC_PDL", 1); halo = geti("HEAL_TC_HALO", 1); bo = geti("HEAL_TC_BO", 0);
-        tma_store = geti("HEAL_TC_TMA_STORE", 1); res_tma = geti("HEAL_TC_RES_TMA", 1); ring = geti("HEAL_TC_RING", 1); deep = geti("HEAL_TC_DEEP", 0); l2promo = geti("HEAL_TC_L2PROMO", 128);
+        tma_store = geti("HEAL_TC_TMA_STORE", 1); res_tma = geti("HEAL_TC_RES_TMA", 1); ring = geti("HEAL_TC_RING", 1); l2promo = geti("HEAL_TC_L2PROMO", 128);
     }
 };
 const TcEnv& tc_env() { static const TcEnv e; return e; }
 
-template <int BLOCK_N, int STAGES, int STG, bool GELU = false>
+template <int BLOCK_N, int STAGES, int STG, bool GELU = false, bool GROUPED = false>
 int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, const CUtensorMap& tmR, const TcP& p_in, cudaStream_t st) {
     TcP p = p_in;
     p.res_tma = (STG >= 2 && p.tma_out && p.res_split && p_in.res_tma) ? 1 : 0;
     const size_t b_tile = p.bdiag ? (size_t)(BLOCK_N / 16) * 512 : (size_t)BLOCK_N * BLOCK_K * 2;
     size_t stage_bytes = (size_t)p.planes * A_TILE_BYTES + (size_t)p.wplanes * b_tile;
     if (p.halo) stage_bytes = (((size_t)p.planes * (p.TW + 2) * 128 + 1023) & ~(size_t)1023) + (size_t)p.wplanes * 3 * b_tile;
-    const size_t scratch = (size_t)BLOCK_M * (BLOCK_N < 64 ? BLOCK_N : 64) * 4;
-    size_t smem = (size_t)STAGES * stage_bytes + (size_t)STG * p.planes * A_TILE_BYTES + scratch + 256;
+    size_t smem = (size_t)STAGES * stage_bytes + (size_t)STG * p.planes * A_TILE_BYTES + 256;
     if (smem > 227 * 1024) return HEAL_ERR_UNSUPPORTED;
+    if (p.tma_out && p.res_split && !p.res_tma) return HEAL_ERR_UNSUPPORTED;
+    if ((p.blockdiag != 0) != GROUPED || (GROUPED && BLOCK_N != 64)) return HEAL_ERR_UNSUPPORTED;    // the staging epilogue adds a split residual only from TMA loads
     static size_t attr_set[HEAL_MAX_DEVICES] = {};
-    if (!heal_ensure_dyn_smem(k_conv2d_tc<BLOCK_N, STAGES, STG, GELU>, 227 * 1024, attr_set)) return HEAL_ERR_LAUNCH;
+    if (!heal_ensure_dyn_smem(k_conv2d_tc<BLOCK_N, STAGES, STG, GELU, GROUPED>, 227 * 1024, attr_set)) return HEAL_ERR_LAUNCH;
     int total = p.m_tiles * p.n_tiles;
     int grid = total < HEAL_NUM_SMS ? total : HEAL_NUM_SMS;
     if (grid < 1) return HEAL_ERR_UNSUPPORTED;
@@ -556,12 +479,20 @@ int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap&
         attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         attr[0].val.programmaticStreamSerializationAllowed = 1;
         cfg.attrs = attr; cfg.numAttrs = 1;
-        cudaError_t e = cudaLaunchKernelEx(&cfg, k_conv2d_tc<BLOCK_N, STAGES, STG, GELU>, tmA, tmB, tmO, tmR, p);
+        cudaError_t e = cudaLaunchKernelEx(&cfg, k_conv2d_tc<BLOCK_N, STAGES, STG, GELU, GROUPED>, tmA, tmB, tmO, tmR, p);
         heal_launch_counter_add(1);
         return e == cudaSuccess ? HEAL_OK : HEAL_ERR_LAUNCH;
     }
-    k_conv2d_tc<BLOCK_N, STAGES, STG, GELU><<<grid, TC_THREADS, smem, st>>>(tmA, tmB, tmO, tmR, p);
+    k_conv2d_tc<BLOCK_N, STAGES, STG, GELU, GROUPED><<<grid, TC_THREADS, smem, st>>>(tmA, tmB, tmO, tmR, p);
     return heal_check_launch();
+}
+
+// 64 output channels per tile: halo tiles with unpacked weights have 81 KiB stages, every other one at most 48 KiB
+template <bool GROUPED>
+int launch_tc64(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, const CUtensorMap& tmR, const TcP& p, cudaStream_t st) {
+    const bool big = p.halo && !p.bdiag;
+    if (!p.tma_out) return big ? launch_tc<64, 2, 0, false, GROUPED>(tmA, tmB, tmO, tmR, p, st) : launch_tc<64, 4, 0, false, GROUPED>(tmA, tmB, tmO, tmR, p, st);
+    return big ? launch_tc<64, 2, 2, false, GROUPED>(tmA, tmB, tmO, tmR, p, st) : launch_tc<64, 3, 2, false, GROUPED>(tmA, tmB, tmO, tmR, p, st);
 }
 
 }  // namespace
@@ -721,9 +652,8 @@ extern "C" int heal_conv2d_tc(const void* in_split, size_t in_plane_stride, int 
             p.res_tma = 1;
         }
     }
-    // a split residual under the TMA-store epilogue is either TMA-loaded (STG == 3) or register-prefetched (halo, <64,2,1>)
-    if (p.tma_out && res_split && !res_tma_ok && !p.halo) p.tma_out = 0;
-    if (p.halo && p.bdiag) p.res_tma = 0;      // <64,4,1>: register prefetch
+    // the TMA-store epilogue adds a split residual from a TMA-loaded copy in its staging buffer; otherwise the direct stores do
+    if (p.tma_out && res_split && !res_tma_ok) p.tma_out = 0;
     cudaStream_t st = (cudaStream_t)stream_;
     const int kblocks = (blockdiag ? 1 : p.kc_blocks) * taps;
     // grouped 3x3 on maps at least 128 pixels wide: the row-ring kernel (conv3x3_ring.cu) reads every input row and the weights
@@ -738,24 +668,20 @@ extern "C" int heal_conv2d_tc(const void* in_split, size_t in_plane_stride, int 
     if (relu == 2) {        // GELU: 1x1 / 3x3 convs with >= 128 output channels and no residual (ConvNeXt pwconv1: dim -> 4 dim)
         if (block_n != 128 || res_split || res_f32) return HEAL_ERR_UNSUPPORTED;
         if (!p.tma_out) return launch_tc<128, 3, 0, true>(tmA, tmB, tmO, tmR, p, st);
-        return kblocks <= 4 ? launch_tc<128, 2, 2, true>(tmA, tmB, tmO, tmR, p, st) : launch_tc<128, 2, 1, true>(tmA, tmB, tmO, tmR, p, st);
+        return kblocks <= 4 ? launch_tc<128, 2, 2, true>(tmA, tmB, tmO, tmR, p, st) : launch_tc<128, 3, 1, true>(tmA, tmB, tmO, tmR, p, st);
     }
-    // Configurations (stages, staging buffers) are sized to the 227 KiB of shared memory per block together with the
-    // 32 KiB fp32 accumulator scratch (split operands; planes == 1 needs less).
+    // Configurations (stages, staging buffers) are sized to the 227 KiB of shared memory per block (split operands; planes == 1
+    // needs less).  A split residual needs two staging buffers (STG >= 2): the next chunk's residual is loaded into one while the
+    // other is drained.  Long-K layers get three stages; short-K layers are bound by the output stream and get two staging
+    // buffers instead.
     switch (block_n) {
         case 16: return launch_tc<16, 4, 0>(tmA, tmB, tmO, tmR, p, st);
         case 32: return launch_tc<32, 4, 0>(tmA, tmB, tmO, tmR, p, st);
         case 64:
-            // halo: 81 KiB stages; a split residual is register-prefetched by the <64,2,1> epilogue
-            if (p.halo && p.bdiag && p.tma_out) return launch_tc<64, 3, 1>(tmA, tmB, tmO, tmR, p, st);     // 45 KiB stages
-            if (p.halo) return p.tma_out ? launch_tc<64, 2, 1>(tmA, tmB, tmO, tmR, p, st) : launch_tc<64, 2, 0>(tmA, tmB, tmO, tmR, p, st);
-            if (p.bdiag && p.tma_out && !res_tma_ok) return launch_tc<64, 3, 2>(tmA, tmB, tmO, tmR, p, st);   // 36 KiB stages
-            if (res_tma_ok) return launch_tc<64, 2, 3>(tmA, tmB, tmO, tmR, p, st);
-            return p.tma_out ? launch_tc<64, 2, 2>(tmA, tmB, tmO, tmR, p, st) : launch_tc<64, 4, 0>(tmA, tmB, tmO, tmR, p, st);
-        default:
+            return blockdiag ? launch_tc64<true>(tmA, tmB, tmO, tmR, p, st) : launch_tc64<false>(tmA, tmB, tmO, tmR, p, st);
+        default:                                                       // 64 KiB stages
             if (!p.tma_out) return launch_tc<128, 3, 0>(tmA, tmB, tmO, tmR, p, st);
-            if (res_tma_ok) return launch_tc<128, 2, 2>(tmA, tmB, tmO, tmR, p, st);
-            // HEAL_TC_DEEP=1 (experiment): one staging buffer also for the short-K layers
-            return (kblocks <= 4 && env.deep != 1) ? launch_tc<128, 2, 2>(tmA, tmB, tmO, tmR, p, st) : launch_tc<128, 2, 1>(tmA, tmB, tmO, tmR, p, st);
+            if (res_tma_ok || kblocks <= 4) return launch_tc<128, 2, 2>(tmA, tmB, tmO, tmR, p, st);
+            return launch_tc<128, 3, 1>(tmA, tmB, tmO, tmR, p, st);
     }
 }

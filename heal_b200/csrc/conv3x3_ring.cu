@@ -14,10 +14,10 @@
 // Output row h needs ring rows h-1, h, h+1: the three horizontal taps are row-shifted descriptors of the same ring row (the
 // swizzle is a function of the absolute shared-memory address), so one new row per output row is all that is loaded.
 // Precision and MMA forms are those of conv2d_tc.cu: a_hi x [b_hi | b_lo] as one N = 32 MMA plus a_lo x b_hi as an N = 16 MMA
-// per 16-channel sub-block and tap, fp32 accumulation in registers.  Roles: warpgroup 0 = TMA producer (warp 0); warpgroups 1
-// and 2 = the M = 64 wgmma of one half of the row tile each, then the epilogue of the whole row (accumulators transposed
-// through an fp32 scratch that shares the bytes of the output staging tile, bias, ReLU, hi/lo split, swizzled staging, one
-// TMA tensor store per row).
+// into separate registers per 16-channel sub-block and tap, fp32 accumulation in registers, folded in the same order.  Roles:
+// warpgroup 0 = TMA producer (warp 0); warpgroups 1 and 2 = the M = 64 wgmma of one half of the row tile each, then the
+// epilogue of their half straight from the accumulator fragment (bias, ReLU, hi/lo split into the swizzled staging tile), one
+// TMA tensor store per row.
 #include <cuda.h>
 #include "common.cuh"
 #include "tc_prims.cuh"
@@ -30,13 +30,12 @@ constexpr int RG_TW = 128;                          // output pixels per row til
 constexpr int RG_ROW_PLANE = (RG_TW + 2) * 128;     // one plane of one ring row: 130 pixels x 64 channels bf16
 constexpr int RG_STG_PLANE = RG_TW * 128;           // one plane of the output staging tile
 constexpr int RG_MAX_SLOTS = 8;
-constexpr int RG_SCRATCH = RG_TW * 64 * 4;          // fp32 accumulator scratch [128 rows][64 channels]
 constexpr int RG_SMEM_LIMIT = 227 * 1024;
 
 __host__ __device__ inline int rg_slot_bytes(int planes) { return (planes * RG_ROW_PLANE + 1023) & ~1023; }
 __host__ __device__ inline int rg_wrow_bytes(int wplanes) { return 3 * 4 * wplanes * 512; }   // one kernel row: [3 taps][4 sub-blocks][plane][16][32 B]
-// output staging tile, also the accumulator scratch
-__host__ __device__ inline int rg_stg_bytes(int planes) { return planes * RG_STG_PLANE > RG_SCRATCH ? planes * RG_STG_PLANE : RG_SCRATCH; }
+// output staging tile
+__host__ __device__ inline int rg_stg_bytes(int planes) { return planes * RG_STG_PLANE; }
 
 __global__ void __launch_bounds__(RG_THREADS, 1)
 k_gconv3x3_ring(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -106,20 +105,22 @@ k_gconv3x3_ring(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         // ============================== consumers: wgmma + epilogue ===============
         regs_inc<232>();
         const int wg = (warp >> 2) - 1;                 // MMAs: pixels [64 wg, 64 wg + 64) of the row tile
-        const int quarter = warp & 3;
-        const int chalf = (warp - 4) >> 2;              // epilogue: which 32 of the 64 channels this warp drains
-        const int row = quarter * 32 + lane;            // epilogue: pixel within the row tile
-        const uint32_t srow = stg + (uint32_t)(row * 128);
-        float bv[32];
+        // accumulator fragment of this thread (tc_prims.cuh): pixels frow and frow + 8, channels 8 j + fcol, +1 of every 8-channel
+        // group j; both pixels have the 128B-swizzle phase fswz in the staging tile
+        const int ft = threadIdx.x & 127;
+        const int frow = 64 * wg + 16 * (ft >> 5) + ((ft & 31) >> 2), fcol = 2 * (ft & 3);
+        const int fswz = (ft >> 2) & 7;
+        const uint32_t row0 = stg + (uint32_t)(frow * 128 + 2 * fcol);      // pixel frow + 8 is 1024 B further
+        float2 bv[8];
 #pragma unroll
-        for (int g = 0; g < 8; ++g) {
-            float4 b4 = p.bias ? __ldg(reinterpret_cast<const float4*>(p.bias + cb * 64 + chalf * 32) + g) : make_float4(0.f, 0.f, 0.f, 0.f);
-            bv[4 * g] = b4.x; bv[4 * g + 1] = b4.y; bv[4 * g + 2] = b4.z; bv[4 * g + 3] = b4.w;
-        }
+        for (int j = 0; j < 8; ++j)
+            bv[j] = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + cb * 64 + 8 * j + fcol)) : make_float2(0.f, 0.f);
         const uint32_t tap_bytes = (uint32_t)(4 * p.wplanes * 512), sub_bytes = (uint32_t)(p.wplanes * 512);
-        float d[64];
+        float d[64], e[32];                              // e: a_lo*b_hi (or a_hi*b_hi with one weight plane) in registers of its own
 #pragma unroll
         for (int i = 0; i < 64; ++i) d[i] = 0.f;
+#pragma unroll
+        for (int i = 0; i < 32; ++i) e[i] = 0.f;
         mbar_wait(bar_w, 0);
         int waited = 0;
         for (int t = 0; t < rows; ++t) {
@@ -138,9 +139,9 @@ k_gconv3x3_ring(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                         const uint64_t bd = gmma_desc_sw32(bs + k * sub_bytes);
                         if (wsplit) {
                             wgmma_bf16<32>(d + 16 * k, a_hi, bd, f0);                                    // [a_hi*b_hi | a_hi*b_lo]
-                            if (split) wgmma_bf16<16>(d + 16 * k, gmma_desc_sw128(al + k * 32), bd, 1u); // += a_lo*b_hi
+                            if (split) wgmma_bf16<16>(e + 8 * k, gmma_desc_sw128(al + k * 32), bd, f0);  // a_lo*b_hi
                         } else {
-                            wgmma_bf16<16>(d + 8 * k, a_hi, bd, f0);
+                            wgmma_bf16<16>(e + 8 * k, a_hi, bd, f0);     // e: every MMA on a register array has one shape
                         }
                     }
                 }
@@ -149,39 +150,33 @@ k_gconv3x3_ring(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             wgmma_wait<0>();
             __syncwarp();
             if (lane == 0) mbar_arrive(bar_empty + 8 * (t % slots));    // input row h-1 is not needed by any later output row
-            if (wsplit) {          // [main16 | aux16] per sub-block -> 64 logical columns
+            if (wsplit) {          // [main16 | aux16] per sub-block + a_lo*b_hi -> 64 logical columns (the fold of k_conv2d_tc)
 #pragma unroll
                 for (int k = 0; k < 4; ++k)
 #pragma unroll
-                    for (int q = 0; q < 8; ++q) d[8 * k + q] = d[16 * k + q] + d[16 * k + 8 + q];
+                    for (int q = 0; q < 8; ++q)
+                        d[8 * k + q] = d[16 * k + q] + (split ? d[16 * k + 8 + q] + e[8 * k + q] : d[16 * k + 8 + q]);
+            } else {
+#pragma unroll
+                for (int i = 0; i < 32; ++i) d[i] = e[i];
             }
-            // the previous row's TMA store has finished reading the staging tile, which now takes the accumulators
+            // the previous row's TMA store has finished reading the staging tile
             if (warp == 4 && lane == 0) bulk_wait_read<0>();
             epi_bar(1);
-            frag_to_scratch<32, 64>(d, stg, 64 * wg, 0);
-            epi_bar(1);
-            uint32_t raw[32];
-            scratch_row<64, 32>(stg, row, chalf * 32, raw);
-            uint32_t hw[4][4], lw[4][4];
+            // bias, ReLU, hi/lo split straight from the fragment into its swizzled slots of the staging tile
 #pragma unroll
-            for (int g8 = 0; g8 < 4; ++g8) {
-                float v[8], lo[8];
+            for (int j = 0; j < 8; ++j) {
+                float v[4] = {d[4 * j] + bv[j].x, d[4 * j + 1] + bv[j].y, d[4 * j + 2] + bv[j].x, d[4 * j + 3] + bv[j].y};
+                if (p.relu) {
 #pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    v[j] = __uint_as_float(raw[g8 * 8 + j]) + bv[g8 * 8 + j];
-                    if (p.relu) v[j] = fmaxf(v[j], 0.f);
-                    lo[j] = v[j] - __bfloat162float(__float2bfloat16_rn(v[j]));
+                    for (int i = 0; i < 4; ++i) v[i] = fmaxf(v[i], 0.f);
                 }
-#pragma unroll
-                for (int j = 0; j < 4; ++j) { hw[g8][j] = pack_bf16(v[2 * j], v[2 * j + 1]); lw[g8][j] = pack_bf16(lo[2 * j], lo[2 * j + 1]); }
-            }
-            epi_bar(1);            // every scratch read is done before the staging tile is overwritten
-#pragma unroll
-            for (int g8 = 0; g8 < 4; ++g8) {
-                const uint32_t chunk16 = (uint32_t)(((chalf * 4 + g8) ^ (row & 7)) * 16);      // 128B swizzle
-                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(srow + chunk16), "r"(hw[g8][0]), "r"(hw[g8][1]), "r"(hw[g8][2]), "r"(hw[g8][3]) : "memory");
-                if (split)
-                    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(srow + RG_STG_PLANE + chunk16), "r"(lw[g8][0]), "r"(lw[g8][1]), "r"(lw[g8][2]), "r"(lw[g8][3]) : "memory");
+                const uint32_t a0 = row0 + (uint32_t)((j ^ fswz) << 4);
+                sts_b32(a0, pack_bf16(v[0], v[1])); sts_b32(a0 + 1024, pack_bf16(v[2], v[3]));
+                if (split) {
+                    sts_b32(a0 + RG_STG_PLANE, pack_bf16(bf16_rest(v[0]), bf16_rest(v[1])));
+                    sts_b32(a0 + RG_STG_PLANE + 1024, pack_bf16(bf16_rest(v[2]), bf16_rest(v[3])));
+                }
             }
             fence_async_smem();
             epi_bar(2);

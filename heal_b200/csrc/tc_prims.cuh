@@ -122,7 +122,7 @@ __device__ __forceinline__ void regs_dec() { asm volatile("setmaxnreg.dec.sync.a
 template <int R>
 __device__ __forceinline__ void regs_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
-// Accumulator transposition through shared memory.  The epilogues work one output ROW per thread (32 consecutive channels),
+// Accumulator transposition through shared memory (spconv_tc.cu).  Its epilogue works one output ROW per thread (32 consecutive channels),
 // the wgmma fragment spreads a row over 4 lanes; a chunk of SW (16, 32 or 64) columns of the 128-row tile goes through an
 // fp32 scratch [128 rows][SW] whose 16-byte slots are XOR-swizzled by row (conflict-free row reads).
 template <int SW>
@@ -179,6 +179,17 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
     __nv_bfloat162 t = __floats2bfloat162_rn(a, b);
     return *reinterpret_cast<uint32_t*>(&t);
 }
+// the two halves of a packed bf16 pair (low half = lower address) as fp32
+__device__ __forceinline__ float bf16_lo_f(uint32_t w) { return __uint_as_float(w << 16); }
+__device__ __forceinline__ float bf16_hi_f(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }
+// what the bf16 rounding of v leaves: the lo plane of the split-bf16 pair (hi = bf16(v), lo = bf16(v - hi))
+__device__ __forceinline__ float bf16_rest(float v) { return v - __bfloat162float(__float2bfloat16_rn(v)); }
+__device__ __forceinline__ uint32_t lds_b32(uint32_t a) {
+    uint32_t v;
+    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
+    return v;
+}
+__device__ __forceinline__ void sts_b32(uint32_t a, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
 
 // 16-byte Ampere-style async copy global -> shared; src_bytes = 0 zero-fills the destination (used for gather rows that miss)
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {

@@ -1,9 +1,10 @@
 """Stand-alone launcher of the four dominant conv shapes of the C2 frame, for `ncu --set full` captures
 (keeps the report small; the launch list of the full frame comes from `bench.py --no-graph`).
-  1. shrink conv 3x3 384->256 @256x256 (N=1)        k_conv2d_tc<128,3>
-  2. per-agent ResNet conv 3x3 64->64 @256x256 (N=1) k_conv2d_tc<64,4>
-  3. ResNeXt level-0 conv1 1x1 64->128 @256x256      k_conv2d_tc<128,3>
-  4. ResNeXt level-0 grouped 3x3 (32 groups, 128 ch) k_conv2d_tc<64,4> (block-diagonal)
+  1. shrink conv 3x3 384->256 @256x256 (N=1)        k_conv2d_tc<128,3,1>
+  2. per-agent ResNet conv 3x3 64->64 @256x256 (N=1) k_conv2d_tc<64,2,2> (halo)
+  3. ResNeXt level-0 conv1 1x1 64->128 @256x256      k_conv2d_tc<128,2,2>
+  4. ResNeXt level-0 grouped 3x3 (32 groups, 128 ch) k_gconv3x3_ring (k_conv2d_tc<64,3,2,false,true> with HEAL_TC_RING=0)
+(template arguments: BLOCK_N, STAGES, staging buffers[, GELU, GROUPED])
 """
 import os
 import sys

@@ -9,7 +9,8 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-SHAPES = [("shrink3x3_384_256_n1", 384, 256, 3, 1, 1), ("res3x3_64_64_n5_res", 64, 64, 3, 1, 5), ("l0_1x1_64_128_n5", 64, 128, 1, 1, 5),
+SHAPES = [("shrink3x3_384_256_n1", 384, 256, 3, 1, 1), ("shrink3x3_256_256_n1", 256, 256, 3, 1, 1),
+          ("res3x3_64_64_n5", 64, 64, 3, 1, 5), ("res3x3_64_64_n5_res", 64, 64, 3, 1, 5), ("l0_1x1_64_128_n5", 64, 128, 1, 1, 5),
           ("l0_1x1_128_64_n5_res", 128, 64, 1, 1, 5), ("l0_grouped_128_n5", 128, 128, 3, 32, 5), ("l1_1x1_256_128_n5_128px_res", 256, 128, 1, 1, 5),
           ("l1_grouped_256_n5_128px", 256, 256, 3, 32, 5),
           ("l2_1x1_256_512_n5_64px", 256, 512, 1, 1, 5), ("l2_1x1_512_256_n5_64px_res", 512, 256, 1, 1, 5), ("l2_grouped_512_n5_64px", 512, 512, 3, 32, 5)]
