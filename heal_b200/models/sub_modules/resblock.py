@@ -76,7 +76,20 @@ class Bottleneck(nn.Module):
 
     out_channels = property(lambda self: self.conv3.out_channels)
 
+    def _fused_eligible(self, x) -> bool:
+        """The shapes ops.bottleneck_tc runs: PyramidFusion's level-0 blocks (64 -> 128 -> 64, 32 groups, stride 1)."""
+        from ... import engine
+        c1, c2, c3 = self.conv1, self.conv2, self.conv3
+        return (isinstance(x, ops.Act) and x.fmt == engine.act_fmt() and engine.PRECISION in ("tc32", "bf16")
+                and not engine.BF16_WEIGHTS and self.downsample is None and c2.stride == (1, 1) and c2.groups == 32
+                and c1.in_channels == x.C == c3.out_channels == 64 and c1.out_channels == c2.out_channels == c3.in_channels == 128
+                and c2.in_channels == 128)
+
     def forward_nhwc(self, x, out=None):
+        if self._fused_eligible(x) and (out is None or out.fmt == x.fmt):
+            from ... import engine
+            pcs = [engine.packed(c, b, True, kind="tc2") for c, b in ((self.conv1, self.bn1), (self.conv2, self.bn2), (self.conv3, self.bn3))]
+            return ops.bottleneck_tc(x, *pcs, out=out)
         idt = x
         if self.downsample is not None:
             idt = conv_bn_act(x, self.downsample[0], self.downsample[1], relu=False)

@@ -588,6 +588,30 @@ def conv2d_tc(x: Act, pc: PackedConvTC, residual: Optional[Act] = None, out: Opt
     return out, out_f32
 
 
+def bottleneck_tc(x: Act, pc1: PackedConvTC, pc2: PackedConvTC, pc3: PackedConvTC, out: Optional[Act] = None,
+                  out_coffset: int = 0) -> Act:
+    """ResNeXt bottleneck ReLU(conv3(conv2(conv1(x))) + x) in one kernel (64 -> 128 -> 64 channels, grouped 3x3, stride 1):
+    bit-identical to conv2d_tc(pc1) -> conv2d_tc(pc2) -> conv2d_tc(pc3, residual=x).  x: Act 'split' or 'bf16'; the packed
+    weights carry both planes.  `out` (optional, x's format): written at channels [out_coffset, out_coffset + 64)."""
+    _need_cuda(pc1.w, pc2.w_diag, pc3.w)
+    assert x.planes in (1, 2) and pc1.planes == pc2.planes == pc3.planes == 2
+    assert (pc1.kh, pc1.cin, pc1.cout, pc3.kh, pc3.cin, pc3.cout) == (1, x.C, 2 * x.C, 1, 2 * x.C, x.C)
+    assert pc2.blockdiag and pc2.kh == 3 and pc2.stride == 1 and pc2.cin == 2 * x.C
+    N, H, W, C = x.N, x.H, x.W, x.C
+    if out is None:
+        out = act_empty(N, H, W, C, x.fmt, x.device)
+    assert out.fmt == x.fmt and (out.N, out.H, out.W) == (N, H, W) and out_coffset + C <= out.C
+    flops = 2.0 * N * H * W * (C * 2 * C + 2 * C * (2 * C // pc2.groups) * 9 + 2 * C * C)
+    epb = 2.0 * x.planes
+    nbytes = 2.0 * N * H * W * C * epb + 2.0 * (pc1.w.numel() + pc2.w_diag.numel() + pc3.w.numel())
+    with _Prof("conv_tc_bottleneck", flops, nbytes):
+        rc = lib.heal_bottleneck_tc(_p(x.t), x.plane_stride, N, H, W, C, x.cstride,
+                                    _p(pc1.w), _p(pc1.bias), _p(pc2.w_diag), _p(pc2.bias), _p(pc3.w), _p(pc3.bias),
+                                    x.planes, pc1.planes, _p(out.t), out.plane_stride, out.cstride, out_coffset, _stream())
+    check(rc, "heal_bottleneck_tc")
+    return out
+
+
 # ------------------------------------------------------------------------------------------------
 # ConvNeXt aligner front half, ResNet-stem max pooling
 # ------------------------------------------------------------------------------------------------

@@ -148,6 +148,16 @@ int heal_conv2d_tc(const void* in_split, size_t in_plane_stride, int N, int H, i
                    float* out_f32, int out32_cstride, int out32_coffset,
                    int Ho, int Wo, int Cout, int upsample, int relu, void* stream);
 
+/* ---- ResNeXt bottleneck, fused (PyramidFusion level 0) ------------------------------------------
+ * y = ReLU(conv3(ReLU(conv2(ReLU(conv1(x))))) + x) for the stride-1 Bottleneck with C = 64 input / output channels, width 128,
+ * 32 groups and no downsample (BN folded into each conv), as one kernel: the width-128 intermediates stay on chip.  The three
+ * weights are the packings heal_conv2d_tc takes for those convs (w_planes = 2): w1 [2][128][64], w2_diag [2][9*128][16] (the
+ * diagonal sub-blocks of the grouped conv), w3 [2][64][128]; biases fp32.  planes 2 (split-bf16) or 1 (bf16).  The output is
+ * bit-identical to the three heal_conv2d_tc launches and may be a channel slice [out_coffset, out_coffset + 64) of a wider map. */
+int heal_bottleneck_tc(const void* x, size_t x_plane_stride, int N, int H, int W, int C, int x_cstride,
+                       const void* w1, const float* b1, const void* w2_diag, const float* b2, const void* w3, const float* b3,
+                       int planes, int w_planes, void* out, size_t out_plane_stride, int out_cstride, int out_coffset, void* stream);
+
 /* ---- PyramidFusion weighted fuse of one level -------------------------------------------------
  * replaces weighted_fuse (opencood/models/fuse_modules/pyramid_fuse.py:17-63) incl. both
  * warp_affine_simple calls (torch_transformation_utils.py:323-332), score = sigmoid(occ)+1e-4
