@@ -46,6 +46,10 @@ SIGNATURES = {
     "heal_maxpool3x3s2": (_i, [_ap, _i, _i, _i, _i, _i, _ap, _vp]),
     "heal_pyramid_fuse_level": (_i, [_ap, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _ap, _vp]),
     "heal_att_fuse": (_i, [_ap, _vp, _i, _i, _i, _i, _ap, _vp]),
+    "heal_max_fuse": (_i, [_ap, _vp, _i, _i, _i, _i, _ap, _vp]),
+    "heal_warp_affine": (_i, [_ap, _vp, _vp, _i, _i, _i, _i, _ap, _vp]),
+    "heal_v2v_aggregate": (_i, [_ap, _ap, _ap, _vp, _vp, _i, _i, _i, _i, _i, _i, _ap, _vp]),
+    "heal_gru_gate": (_i, [_ap, _c.c_longlong, _i, _ap, _vp]),
     "heal_act_convert": (_i, [_ap, _ap, _sz, _i, _vp]),
     "heal_postprocess_workspace": (_sz, [_i, _i, _i, _i]),
     "heal_box_decode_nms": (_i, [_ap, _ap, _ap, _vp, _i, _i, _i, _c.c_float, _c.c_float, _i, _vp, _i, _c.c_float, _i,

@@ -4,9 +4,12 @@
 //       (score = sigmoid(occ) + 1e-4, camera crop mask in eval mode)
 //   heal_att_fuse           : warp -> per-pixel scaled dot-product attention over agents, ego row only
 //       reference: opencood/models/fuse_modules/fusion_in_one.py:126-151 (AttFusion), :41-45
-// Both fold warp_affine_simple (torch_transformation_utils.py:323-332 = F.affine_grid with an fp64
+//   heal_max_fuse           : warp -> max over agents (MaxFusion, fusion_in_one.py:87-124)
+// All three fold warp_affine_simple (torch_transformation_utils.py:323-332 = F.affine_grid with an fp64
 // theta, cast to fp32, then F.grid_sample bilinear / zeros padding) into the fusion so the warped
 // per-agent maps never exist in HBM.
+//   heal_warp_affine, heal_v2v_aggregate, heal_gru_gate : the non-conv steps of V2VNetFusion (fusion_in_one.py:203-318),
+//       whose message and GRU convolutions run on the conv engine between them.
 #include "common.cuh"
 #include "../../include/heal_b200.h"
 
@@ -393,6 +396,118 @@ k_att_fuse_split8(AttP p) {
     }
 }
 
+// ---- MaxFusion / V2VNetFusion (fusion_in_one.py:87-124, :203-318) ---------------------------------------------------------
+// One thread per (image, pixel, 4-channel chunk); blockIdx.y is the image inside the launch.  Every thread recomputes its taps
+// with make_tap (a few fp64 FMAs), so the arithmetic per tap is the one the attention / pyramid kernels use.
+
+// bilinear sample of 4 channels of one image, zeros padding: FMA over the in-bounds taps in (nw, ne, sw, se) order
+__device__ __forceinline__ float4 tap_sample4(const ActV& a, long long img_pix0, const Tap& t, int c) {
+    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        if (t.off[k] >= 0) {
+            const float4 v = act_load4(a, (size_t)(img_pix0 + t.off[k]), c);
+            const float w = t.w[k];
+            s.x = fmaf(v.x, w, s.x); s.y = fmaf(v.y, w, s.y); s.z = fmaf(v.z, w, s.z); s.w = fmaf(v.w, w, s.w);
+        }
+    }
+    return s;
+}
+
+struct MaxP { ActV feat; const double* theta; ActV out; int n, H, W, C, align; };
+
+// out = max over agents of warp(feat_j, theta_j).  A pixel warped in from outside agent j's map samples 0, and that 0 takes part
+// in the max (torch.max over the warped stack).
+__global__ void __launch_bounds__(256) k_max_fuse(MaxP p) {
+    const int chunks = p.C >> 2, HW = p.H * p.W;
+    const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= (long long)HW * chunks) return;
+    const int pix = (int)(g / chunks), c = (int)(g % chunks) * 4;
+    float4 m = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int j = 0; j < p.n; ++j) {
+        const Tap t = make_tap(p.theta + 6 * j, pix / p.W, pix % p.W, p.H, p.W, p.align);
+        const float4 v = tap_sample4(p.feat, (long long)j * HW, t, c);
+        if (j == 0) m = v;
+        else { m.x = fmaxf(m.x, v.x); m.y = fmaxf(m.y, v.y); m.z = fmaxf(m.z, v.z); m.w = fmaxf(m.w, v.w); }
+    }
+    act_store4(p.out, (size_t)pix, c, m);
+}
+
+constexpr int WARP_BATCH = 256;    // output images per heal_warp_affine launch (source indices travel in the parameter block)
+
+struct WarpP { ActV src; const double* theta; ActV out; int H, W, C, k0; int src_img[WARP_BATCH]; };
+
+// out image k0 + y = grid_sample(src image src_img[y], theta[k0 + y])
+__global__ void __launch_bounds__(256) k_warp_affine(WarpP p) {
+    const int chunks = p.C >> 2, HW = p.H * p.W;
+    const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= (long long)HW * chunks) return;
+    const int pix = (int)(g / chunks), c = (int)(g % chunks) * 4;
+    const int k = p.k0 + blockIdx.y;
+    const Tap t = make_tap(p.theta + 6 * (long long)k, pix / p.W, pix % p.W, p.H, p.W, 0);
+    act_store4(p.out, (size_t)k * HW + pix, c, tap_sample4(p.src, (long long)p.src_img[blockIdx.y] * HW, t, c));
+}
+
+constexpr int AGG_BATCH = 64;      // updated nodes per heal_v2v_aggregate launch
+
+struct AggP {
+    ActV q, pn, x, out; const double* theta;
+    int H, W, C, agg_max, gru, u0;
+    int4 node[AGG_BATCH];          // (x image, P image, first pair row, number of neighbours n) of updated node u0 + y
+};
+
+// One V2VNet node update.  msg_ij = mask_ij * (Q_ij + P_i) with Q_ij = W[:, :C] (*) warp(x_j, theta_ij) and P_i = W[:, C:] (*) x_i
+// + b: the message conv of cat[warp(x_j), x_i] split along K, so P_i is computed once per node.  mask_ij = warp(ones, theta_ij) is
+// the sum of the in-bounds tap weights (fractional on border pixels).  agg_i = mean over all n neighbours (self included, /n) or
+// their max; with the GRU the output is the GRU conv input [x_i | agg_i], without it the next node feature x_i + agg_i.
+__global__ void __launch_bounds__(256) k_v2v_aggregate(AggP p) {
+    const int chunks = p.C >> 2, HW = p.H * p.W;
+    const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= (long long)HW * chunks) return;
+    const int pix = (int)(g / chunks), c = (int)(g % chunks) * 4;
+    const int4 nd = p.node[blockIdx.y];
+    const int u = p.u0 + blockIdx.y;
+    const float4 pi = act_load4(p.pn, (size_t)nd.y * HW + pix, c);
+    float4 acc = p.agg_max ? make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY) : make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int j = 0; j < nd.w; ++j) {
+        const long long row = (long long)nd.z + j;
+        const Tap t = make_tap(p.theta + 6 * row, pix / p.W, pix % p.W, p.H, p.W, 0);
+        float m = 0.f;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) m += (t.off[k] >= 0) ? t.w[k] : 0.f;
+        const float4 q = act_load4(p.q, (size_t)(row * HW + pix), c);
+        const float4 v = make_float4(m * (q.x + pi.x), m * (q.y + pi.y), m * (q.z + pi.z), m * (q.w + pi.w));
+        if (p.agg_max) { acc.x = fmaxf(acc.x, v.x); acc.y = fmaxf(acc.y, v.y); acc.z = fmaxf(acc.z, v.z); acc.w = fmaxf(acc.w, v.w); }
+        else { acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w; }
+    }
+    if (!p.agg_max) {
+        const float inv = (float)nd.w;
+        acc.x /= inv; acc.y /= inv; acc.z /= inv; acc.w /= inv;
+    }
+    const float4 xi = act_load4(p.x, (size_t)nd.x * HW + pix, c);
+    const size_t opix = (size_t)u * HW + pix;
+    if (p.gru) {
+        act_store4(p.out, opix, c, xi);
+        act_store4(p.out, opix, p.C + c, acc);
+    } else {
+        act_store4(p.out, opix, c, make_float4(xi.x + acc.x, xi.y + acc.y, xi.z + acc.z, xi.w + acc.w));
+    }
+}
+
+// ConvGRU cell with a zero hidden state: h' = sigmoid(z) * tanh(c), z = channels [0, C) and c = channels [C, 2C) of the GRU conv
+// output (update-gate rows of conv_gates stacked over conv_can; the reset gate multiplies h = 0 and drops out).
+__global__ void __launch_bounds__(256) k_gru_gate(ActV zc, ActV out, long long npix, int C) {
+    const int chunks = C >> 2;
+    const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= npix * chunks) return;
+    const size_t pix = (size_t)(g / chunks);
+    const int c = (int)(g % chunks) * 4;
+    const float4 z = act_load4(zc, pix, c), cc = act_load4(zc, pix, C + c);
+    const float4 h = make_float4((1.f / (1.f + expf(-z.x))) * tanhf(cc.x), (1.f / (1.f + expf(-z.y))) * tanhf(cc.y),
+                                 (1.f / (1.f + expf(-z.z))) * tanhf(cc.z), (1.f / (1.f + expf(-z.w))) * tanhf(cc.w));
+    act_store4(out, pix, c, h);
+}
+
 }  // namespace
 
 static inline ActV to_view(const heal_act_t* a) {
@@ -459,5 +574,74 @@ extern "C" int heal_att_fuse(const heal_act_t* feat, const double* theta, int n_
         case 3: k_att_fuse<3><<<grid, 256, 0, st>>>(p); break;
         default: k_att_fuse<4><<<grid, 256, 0, st>>>(p); break;
     }
+    return heal_check_launch();
+}
+
+// views read / written 4 channels at a time: 16 B-aligned fp32, 8 B-aligned bf16 planes
+static inline bool aligned4(const heal_act_t* a) {
+    return (a->cstride & 3) == 0 && (a->coffset & 3) == 0 && (a->fmt == 0 || (a->plane_stride & 3) == 0);
+}
+static inline long long grid_x(int H, int W, int C) { return ((long long)H * W * (C / 4) + 255) / 256; }
+
+extern "C" int heal_max_fuse(const heal_act_t* feat, const double* theta, int n_agents, int H, int W, int C,
+                             const heal_act_t* out, void* stream_) {
+    if (!feat || !feat->data || !theta || !out || !out->data || H < 1 || W < 1) return HEAL_ERR_ARG;
+    if (n_agents < 1 || (C & 3) || !aligned4(feat) || !aligned4(out)) return HEAL_ERR_UNSUPPORTED;
+    MaxP p;
+    p.feat = to_view(feat); p.theta = theta; p.out = to_view(out); p.n = n_agents; p.H = H; p.W = W; p.C = C; p.align = 0;
+    k_max_fuse<<<(unsigned)grid_x(H, W, C), 256, 0, (cudaStream_t)stream_>>>(p);
+    return heal_check_launch();
+}
+
+extern "C" int heal_warp_affine(const heal_act_t* src, const int* src_index_host, const double* theta, int n_out,
+                                int H, int W, int C, const heal_act_t* out, void* stream_) {
+    if (!src || !src->data || !src_index_host || !theta || !out || !out->data || n_out < 0 || H < 1 || W < 1) return HEAL_ERR_ARG;
+    if ((C & 3) || !aligned4(src) || !aligned4(out)) return HEAL_ERR_UNSUPPORTED;
+    WarpP p;
+    p.src = to_view(src); p.theta = theta; p.out = to_view(out); p.H = H; p.W = W; p.C = C;
+    int launches = 0;
+    for (int k0 = 0; k0 < n_out; k0 += WARP_BATCH) {
+        const int nb = n_out - k0 < WARP_BATCH ? n_out - k0 : WARP_BATCH;
+        p.k0 = k0;
+        for (int y = 0; y < nb; ++y) {
+            if (src_index_host[k0 + y] < 0) return HEAL_ERR_ARG;
+            p.src_img[y] = src_index_host[k0 + y];
+        }
+        k_warp_affine<<<dim3((unsigned)grid_x(H, W, C), nb), 256, 0, (cudaStream_t)stream_>>>(p);
+        ++launches;
+    }
+    return heal_check_launch(launches);
+}
+
+extern "C" int heal_v2v_aggregate(const heal_act_t* q, const heal_act_t* p_node, const heal_act_t* x, const double* theta,
+                                  const int* nodes_host, int n_nodes, int H, int W, int C, int agg_max, int gru,
+                                  const heal_act_t* out, void* stream_) {
+    if (!q || !q->data || !p_node || !p_node->data || !x || !x->data || !theta || !nodes_host || !out || !out->data) return HEAL_ERR_ARG;
+    if (n_nodes < 0 || H < 1 || W < 1) return HEAL_ERR_ARG;
+    if ((C & 3) || !aligned4(q) || !aligned4(p_node) || !aligned4(x) || !aligned4(out)) return HEAL_ERR_UNSUPPORTED;
+    AggP p;
+    p.q = to_view(q); p.pn = to_view(p_node); p.x = to_view(x); p.out = to_view(out); p.theta = theta;
+    p.H = H; p.W = W; p.C = C; p.agg_max = agg_max ? 1 : 0; p.gru = gru ? 1 : 0;
+    int launches = 0;
+    for (int u0 = 0; u0 < n_nodes; u0 += AGG_BATCH) {
+        const int nb = n_nodes - u0 < AGG_BATCH ? n_nodes - u0 : AGG_BATCH;
+        p.u0 = u0;
+        for (int y = 0; y < nb; ++y) {
+            const int* nd = nodes_host + 4 * (u0 + y);
+            if (nd[0] < 0 || nd[1] < 0 || nd[2] < 0 || nd[3] < 1) return HEAL_ERR_ARG;
+            p.node[y] = make_int4(nd[0], nd[1], nd[2], nd[3]);
+        }
+        k_v2v_aggregate<<<dim3((unsigned)grid_x(H, W, C), nb), 256, 0, (cudaStream_t)stream_>>>(p);
+        ++launches;
+    }
+    return heal_check_launch(launches);
+}
+
+extern "C" int heal_gru_gate(const heal_act_t* zc, long long npix, int C, const heal_act_t* out, void* stream_) {
+    if (!zc || !zc->data || !out || !out->data || npix < 0) return HEAL_ERR_ARG;
+    if ((C & 3) || !aligned4(zc) || !aligned4(out)) return HEAL_ERR_UNSUPPORTED;
+    if (npix == 0) return HEAL_OK;
+    const long long blocks = (npix * (C / 4) + 255) / 256;
+    k_gru_gate<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream_>>>(to_view(zc), to_view(out), npix, C);
     return heal_check_launch();
 }

@@ -1,7 +1,7 @@
 """HeterModelBaseline mirror (opencood/models/heter_model_baseline.py:26-236): per-modality encoder ->
-BaseBEVBackbone -> per-agent shrinker -> single-scale fusion (`fusion_method: att`, AttFusion) -> heads.
-Same ctor argument, state-dict keys and forward(data_dict) -> output_dict contract.  The other fusion_method
-options of the reference (disconet, v2vnet, v2xvit, cobevt, where2comm, who2com) are outside the hot-path scope."""
+BaseBEVBackbone -> per-agent shrinker -> single-scale fusion -> heads.  Same ctor argument, state-dict keys and forward(data_dict) -> output_dict contract.
+`fusion_method`: att (AttFusion), max (F-Cooper MaxFusion) and v2vnet (V2VNetFusion).  disconet cannot be constructed in the
+reference itself; v2xvit, cobevt, where2comm and who2com are outside the hot-path scope."""
 import importlib
 from collections import OrderedDict, Counter
 
@@ -13,7 +13,7 @@ from ..engine import require_eval
 from ..utils.transformation_utils import normalize_pairwise_tfm
 from .sub_modules.base_bev_backbone import BaseBEVBackbone
 from .sub_modules.downsample_conv import DownsampleConv
-from .fuse_modules.fusion_in_one import AttFusion
+from .fuse_modules.fusion_in_one import AttFusion, MaxFusion, V2VNetFusion
 from .heter_pyramid_collab import FusedHeads, HeterPyramidCollab
 
 
@@ -51,10 +51,18 @@ class HeterModelBaseline(nn.Module):
             self.reg_head_single = nn.Conv2d(c, args['anchor_number'] * 7, kernel_size=1)
             self.dir_head_single = nn.Conv2d(c, args['anchor_number'] * args['dir_args']['num_bins'], kernel_size=1)
             self._heads_single = FusedHeads([self.cls_head_single, self.reg_head_single, self.dir_head_single])
-        if args['fusion_method'] == "att":
+        fm = args['fusion_method']
+        if fm == "att":
             self.fusion_net = AttFusion(args['att']['feat_dim'])
+        elif fm == "max":
+            self.fusion_net = MaxFusion()
+        elif fm == "v2vnet":
+            self.fusion_net = V2VNetFusion(args['v2vnet'])
+        elif fm == "disconet":
+            raise NotImplementedError("fusion_method 'disconet': DiscoFusion cannot be constructed in the reference either "
+                                      "(it imports opencood.models.fuse_modules.disco_fuse, which the reference does not ship)")
         else:
-            raise NotImplementedError(f"fusion_method '{args['fusion_method']}' is outside the heal_b200 hot-path scope (att only)")
+            raise NotImplementedError(f"fusion_method '{fm}' is outside the heal_b200 hot-path scope (built: att, max, v2vnet)")
         self.shrink_flag = 'shrink_header' in args
         if self.shrink_flag:
             self.shrink_conv = DownsampleConv(args['shrink_header'])

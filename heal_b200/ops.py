@@ -695,6 +695,82 @@ def att_fuse(feat: Act, theta: torch.Tensor, out: Optional[Act] = None, out_fmt:
     return out
 
 
+def max_fuse(feat: Act, theta: torch.Tensor, out: Optional[Act] = None, out_fmt: Optional[str] = None) -> Act:
+    """MaxFusion of one scene: feat Act (n,H,W,C), theta (n,2,3) f64 -> Act (1,H,W,C) = max_j warp(feat_j, theta_j)."""
+    _need_cuda(theta)
+    n, H, W, C = feat.N, feat.H, feat.W, feat.C
+    th = theta.to(torch.float64).contiguous()
+    assert th.shape == (n, 2, 3)
+    if out is None:
+        out = act_empty(1, H, W, C, out_fmt or feat.fmt, feat.device)
+    assert (out.H, out.W, out.C) == (H, W, C)
+    fv, ov = feat.view(), out.view()
+    with _Prof("max_fuse", 4.0 * n * C * H * W, (n * BPE[feat.fmt] + BPE[out.fmt]) * float(C) * H * W):
+        rc = lib.heal_max_fuse(ctypes.byref(fv), _p(th), n, H, W, C, ctypes.byref(ov), _stream())
+    check(rc, "heal_max_fuse")
+    return out
+
+
+def warp_affine(src: Act, src_index: Sequence[int], theta: torch.Tensor, out: Optional[Act] = None,
+                out_fmt: Optional[str] = None) -> Act:
+    """Batched warp_affine_simple (bilinear, zeros, align_corners=False): out image k = warp(src image src_index[k], theta[k]).
+    src Act (n,H,W,C); theta (K,2,3) f64 on the device; `src_index` a host sequence of K image indices -> Act (K,H,W,C)."""
+    _need_cuda(theta)
+    K, H, W, C = len(src_index), src.H, src.W, src.C
+    th = theta.to(torch.float64).contiguous()
+    assert th.shape == (K, 2, 3) and all(0 <= int(s) < src.N for s in src_index)
+    if out is None:
+        out = act_empty(K, H, W, C, out_fmt or src.fmt, src.device)
+    assert (out.N, out.H, out.W, out.C) == (K, H, W, C)
+    sv, ov = src.view(), out.view()
+    with _Prof("warp_affine", 8.0 * K * C * H * W, K * (BPE[src.fmt] + BPE[out.fmt]) * float(C) * H * W):
+        rc = lib.heal_warp_affine(ctypes.byref(sv), _host_i32(src_index), _p(th), K, H, W, C, ctypes.byref(ov), _stream())
+    check(rc, "heal_warp_affine")
+    return out
+
+
+def v2v_aggregate(q: Act, p_node: Act, x: Act, theta: torch.Tensor, nodes: Sequence[Sequence[int]], agg_max: bool,
+                  gru: bool, out: Optional[Act] = None, out_fmt: Optional[str] = None) -> Act:
+    """V2VNet message aggregation.  nodes[u] = (x image, P image, first pair row r, neighbour count n) of updated node u;
+    pair row r + j holds q = W[:, :C] (*) warp(x_j, theta[r + j]).  Returns Act (U,H,W,2C) = [x | agg] when `gru`, else
+    Act (U,H,W,C) = x + agg; agg = mean_j (agg_max False) or max_j of mask_j * (q[r + j] + p_node[P image])."""
+    _need_cuda(theta)
+    H, W, C, U = x.H, x.W, x.C, len(nodes)
+    th = theta.to(torch.float64).contiguous()
+    assert th.shape == (q.N, 2, 3) and (q.H, q.W, q.C) == (H, W, C) and (p_node.H, p_node.W, p_node.C) == (H, W, C)
+    flat = [int(v) for nd in nodes for v in nd]
+    assert len(flat) == 4 * U
+    cout = 2 * C if gru else C
+    if out is None:
+        out = act_empty(U, H, W, cout, out_fmt or x.fmt, x.device)
+    assert (out.N, out.H, out.W, out.C) == (U, H, W, cout)
+    pairs = float(sum(nd[3] for nd in nodes))
+    qv, pv, xv, ov = q.view(), p_node.view(), x.view(), out.view()
+    with _Prof("v2v_aggregate", 3.0 * pairs * C * H * W,
+               (pairs * BPE[q.fmt] + U * (BPE[p_node.fmt] + BPE[x.fmt]) + U * (cout // C) * BPE[out.fmt]) * float(C) * H * W):
+        rc = lib.heal_v2v_aggregate(ctypes.byref(qv), ctypes.byref(pv), ctypes.byref(xv), _p(th), _host_i32(flat), U, H, W, C,
+                                    1 if agg_max else 0, 1 if gru else 0, ctypes.byref(ov), _stream())
+    check(rc, "heal_v2v_aggregate")
+    return out
+
+
+def gru_gate(zc: Act, out: Optional[Act] = None, out_fmt: Optional[str] = None) -> Act:
+    """Zero-hidden ConvGRU cell output: zc Act (N,H,W,2C) = (update-gate | candidate) conv output -> Act (N,H,W,C)
+    = sigmoid(zc[..., :C]) * tanh(zc[..., C:])."""
+    N, H, W = zc.N, zc.H, zc.W
+    assert zc.C % 2 == 0
+    C = zc.C // 2
+    if out is None:
+        out = act_empty(N, H, W, C, out_fmt or zc.fmt, zc.device)
+    assert (out.N, out.H, out.W, out.C) == (N, H, W, C)
+    zv, ov = zc.view(), out.view()
+    npix = N * H * W
+    with _Prof("gru_gate", 4.0 * npix * C, npix * float(C) * (2 * BPE[zc.fmt] + BPE[out.fmt])):
+        rc = lib.heal_gru_gate(ctypes.byref(zv), npix, C, ctypes.byref(ov), _stream())
+    check(rc, "heal_gru_gate")
+    return out
+
+
 # ------------------------------------------------------------------------------------------------
 # Lift-Splat-Shoot
 # ------------------------------------------------------------------------------------------------

@@ -179,6 +179,32 @@ int heal_pyramid_fuse_level(const heal_act_t* feat, const float* occ, const doub
 int heal_att_fuse(const heal_act_t* feat, const double* theta, int n_agents, int H, int W, int C,
                   const heal_act_t* out, void* stream);
 
+/* MaxFusion.forward for one scene (fusion_in_one.py:87-124): out(H,W,C) = max over j of warp(feat_j, theta[j]).
+ * Pixels warped in from outside agent j's map are 0 and take part in the max.  feat (n,H,W,C), theta (n,2,3) fp64 device;
+ * C, channel strides and offsets multiples of 4. */
+int heal_max_fuse(const heal_act_t* feat, const double* theta, int n_agents, int H, int W, int C,
+                  const heal_act_t* out, void* stream);
+
+/* A batch of warp_affine_simple (bilinear, zeros padding, align_corners=False):
+ * out image k = grid_sample(src image src_index_host[k], theta[k]) for k < n_out.
+ * src_index_host: HOST array of n_out image indices into src (H,W,C maps); theta (n_out,2,3) fp64 device; out (n_out,H,W,C). */
+int heal_warp_affine(const heal_act_t* src, const int* src_index_host, const double* theta, int n_out,
+                     int H, int W, int C, const heal_act_t* out, void* stream);
+
+/* V2VNet message aggregation (fusion_in_one.py:262-300) for n_nodes updated nodes.  nodes_host: HOST array of n_nodes
+ * int quadruples (x image, P image, first pair row r, neighbours n).  For updated node u and j < n:
+ *   msg_j = mask_j * (q[r + j] + p_node[P image]),  mask_j = warp(ones, theta[r + j]) (recomputed from the taps)
+ *   agg   = mean_j msg_j (agg_max = 0, divides by n) or max_j msg_j (agg_max = 1)
+ * gru = 1: out image u (2C channels) = [x | agg]  (the ConvGRU input);  gru = 0: out image u (C channels) = x + agg.
+ * q (pairs,H,W,C) = W[:, :C] (*) warped neighbours; p_node (.,H,W,C) = W[:, C:] (*) x + bias; theta (pairs,2,3) fp64 device. */
+int heal_v2v_aggregate(const heal_act_t* q, const heal_act_t* p_node, const heal_act_t* x, const double* theta,
+                       const int* nodes_host, int n_nodes, int H, int W, int C, int agg_max, int gru,
+                       const heal_act_t* out, void* stream);
+
+/* ConvGRU cell with a zero hidden state (sub_modules/convgru.py:47-68): out(npix,C) = sigmoid(zc[:, :C]) * tanh(zc[:, C:2C]),
+ * zc = the stacked (update gate | candidate) GRU conv output (npix, 2C). */
+int heal_gru_gate(const heal_act_t* zc, long long npix, int C, const heal_act_t* out, void* stream);
+
 /* ---- Lift-Splat-Shoot ------------------------------------------------------------------------
  * heal_lss_cell_index replaces LiftSplatShoot.get_geometry + the index half of voxel_pooling
  * (opencood/models/heter_encoders.py:125-147, :173-185): for every frustum point of every camera image
