@@ -5,10 +5,36 @@
 // HBM-bound: reads the map once (the 7x7 neighbourhood of a pixel is shared through L1/L2 by the warps of a block, which cover
 // 8 x 4 neighbouring pixels), writes it once.  One warp per pixel, lane = channel pair (C = 64) -> every tap is one coalesced
 // 256 B (fp32) row read; mean / variance by warp shuffles, exactly LayerNorm's biased variance.
+// heal_mean_layernorm reuses that LayerNorm after a mean over n_avg consecutive images: CoBEVT's pre-norms (n_avg = 1) and its
+// mlp_head Reduce-mean over the agent slots + LayerNorm (n_avg = L; fusion_in_one.py:401-407).
 #include "common.cuh"
 #include "../../include/heal_b200.h"
 
 namespace {
+
+// LayerNorm over the C channels (C = 64 .. 256, multiple of 64) of one pixel held by one warp: acc[2q], acc[2q + 1] are channels
+// q * 64 + 2 * lane and + 1.  Mean and biased variance by warp shuffles (LayerNorm's definition), then the affine transform.
+// The one LayerNorm of the library: the ConvNeXt front half and CoBEVT's pre-norms / head both end in it.
+__device__ __forceinline__ void warp_layernorm_store(const float (&acc)[8], int C, int lane, const float* lnw, const float* lnb,
+                                                     float eps, const ActV& out, size_t opix) {
+    const int chunks = C / 64;
+    float s = 0.f;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) if (q < chunks) s += acc[2 * q] + acc[2 * q + 1];
+    const float mean = warp_sum(s) / (float)C;
+    float v = 0.f;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) if (q < chunks) { const float d0 = acc[2 * q] - mean, d1 = acc[2 * q + 1] - mean; v += d0 * d0 + d1 * d1; }
+    const float rstd = rsqrtf(warp_sum(v) / (float)C + eps);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+        if (q < chunks) {
+            const int c = q * 64 + 2 * lane;
+            act_store1(out, opix, c, (acc[2 * q] - mean) * rstd * __ldg(lnw + c) + __ldg(lnb + c));
+            act_store1(out, opix, c + 1, (acc[2 * q + 1] - mean) * rstd * __ldg(lnw + c + 1) + __ldg(lnb + c + 1));
+        }
+    }
+}
 
 struct DwLnP {
     ActV in, out;
@@ -50,18 +76,48 @@ k_dwconv_ln(DwLnP p) {
         }
         acc[2 * q] = a0; acc[2 * q + 1] = a1;
     }
-    float s = 0.f;
-    for (int q = 0; q < chunks; ++q) s += acc[2 * q] + acc[2 * q + 1];
-    const float mean = warp_sum(s) / (float)p.C;
-    float v = 0.f;
-    for (int q = 0; q < chunks; ++q) { const float d0 = acc[2 * q] - mean, d1 = acc[2 * q + 1] - mean; v += d0 * d0 + d1 * d1; }
-    const float rstd = rsqrtf(warp_sum(v) / (float)p.C + p.eps);
-    const size_t opix = img + (size_t)y * p.W + x;
-    for (int q = 0; q < chunks; ++q) {
-        const int c = q * 64 + 2 * lane;
-        act_store1(p.out, opix, c, (acc[2 * q] - mean) * rstd * __ldg(p.lnw + c) + __ldg(p.lnb + c));
-        act_store1(p.out, opix, c + 1, (acc[2 * q + 1] - mean) * rstd * __ldg(p.lnw + c + 1) + __ldg(p.lnb + c + 1));
+    warp_layernorm_store(acc, p.C, lane, p.lnw, p.lnb, p.eps, p.out, img + (size_t)y * p.W + x);
+}
+
+struct MeanLnP {
+    ActV in, out;
+    const float* lnw;
+    const float* lnb;
+    long long npix;      // output pixels (n_out * H * W)
+    int HW, C, n_avg;
+    float eps;
+};
+
+// block = 8 warps = 8 output pixels.  Output image o, pixel x = LayerNorm(mean over k < n_avg of input image o * n_avg + k, pixel x)
+// (n_avg = 1: a plain channels-last LayerNorm)
+__global__ void __launch_bounds__(256)
+k_mean_layernorm(MeanLnP p) {
+    const int lane = threadIdx.x & 31;
+    const long long g = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (g >= p.npix) return;
+    const long long o = g / p.HW;
+    const int pix = (int)(g - o * p.HW);
+    const int chunks = p.C / 64;
+    float acc[8];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) { acc[2 * q] = 0.f; acc[2 * q + 1] = 0.f; }
+    for (int k = 0; k < p.n_avg; ++k) {
+        const size_t ip = (size_t)(o * p.n_avg + k) * p.HW + pix;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            if (q < chunks) {
+                const int c = q * 64 + 2 * lane;
+                acc[2 * q] += act_load1(p.in, ip, c);
+                acc[2 * q + 1] += act_load1(p.in, ip, c + 1);
+            }
+        }
     }
+    if (p.n_avg > 1) {
+        const float n = (float)p.n_avg;
+#pragma unroll
+        for (int q = 0; q < 8; ++q) acc[q] /= n;
+    }
+    warp_layernorm_store(acc, p.C, lane, p.lnw, p.lnb, p.eps, p.out, (size_t)g);
 }
 
 // 3x3 / stride-2 / pad-1 max pooling (torchvision ResNet stem), channels-last, thread = (pixel, 4 channels)
@@ -119,5 +175,17 @@ extern "C" int heal_maxpool3x3s2(const heal_act_t* in, int N, int H, int W, int 
     const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
     const long long total = (long long)N * Ho * Wo * (C / 4);
     k_maxpool3s2<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(view_of(in), view_of(out), N, H, W, C, Ho, Wo, depth_to_space_in);
+    return heal_check_launch();
+}
+
+extern "C" int heal_mean_layernorm(const heal_act_t* in, int n_out, int n_avg, int H, int W, int C, const float* ln_weight,
+                                   const float* ln_bias, float eps, const heal_act_t* out, void* stream_) {
+    if (!in || !in->data || !out || !out->data || !ln_weight || !ln_bias || n_out < 0 || n_avg < 1 || H < 1 || W < 1) return HEAL_ERR_ARG;
+    if ((C % 64) || C < 64 || C > 256) return HEAL_ERR_UNSUPPORTED;
+    MeanLnP p;
+    p.in = view_of(in); p.out = view_of(out); p.lnw = ln_weight; p.lnb = ln_bias;
+    p.npix = (long long)n_out * H * W; p.HW = H * W; p.C = C; p.n_avg = n_avg; p.eps = eps;
+    if (p.npix == 0) return HEAL_OK;
+    k_mean_layernorm<<<(unsigned)((p.npix + 7) / 8), 256, 0, (cudaStream_t)stream_>>>(p);
     return heal_check_launch();
 }

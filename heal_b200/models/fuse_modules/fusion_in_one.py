@@ -1,13 +1,14 @@
-"""Fusion operator mirrors of opencood/models/fuse_modules/fusion_in_one.py: AttFusion (:126-151), MaxFusion (:87-124) and
-V2VNetFusion (:203-318), with the reference's `forward(x, record_len, affine_matrix)` signature (NCHW) and `forward_nhwc`
-(conv-engine activations).  DiscoFusion cannot be constructed in the reference (it imports a `disco_fuse` module the reference
-does not ship); V2X-ViT, CoBEVT, Where2comm and Who2com are out of scope (SURVEY.md 2.1 row 14)."""
+"""Fusion operator mirrors of opencood/models/fuse_modules/fusion_in_one.py: AttFusion (:126-151), MaxFusion (:87-124),
+V2VNetFusion (:203-318) and CoBEVT (:374-429), with the reference's `forward(x, record_len, affine_matrix)` signature (NCHW) and
+`forward_nhwc` (conv-engine activations).  DiscoFusion cannot be constructed in the reference (it imports a `disco_fuse` module
+the reference does not ship); V2X-ViT, Where2comm and Who2com are out of scope (SURVEY.md 2.1 row 14)."""
 import numpy as np
 import torch
 import torch.nn as nn
 
 from ... import engine, ops
-from ...engine import conv_bn_act
+from ...engine import conv_bn_act, require_eval
+from .swap_fusion_modules import SwapFusionBlockMask
 
 
 def regroup(x, record_len):
@@ -213,4 +214,112 @@ class V2VNetFusion(nn.Module):
 
     def forward(self, x, record_len, affine_matrix):
         self._check(*x.shape[1:])
+        return ops.act_to_nchw(self.forward_nhwc(ops.to_act(x), record_len, affine_matrix))
+
+
+class CoBEVT(nn.Module):
+    """CoBEVT (fusion_in_one.py:374-429) with the reference's ctor and state-dict keys (`layers.{i}.{window,grid}_{attention,ffd}`,
+    `mlp_head.2` LayerNorm, `mlp_head.3` Linear; the einops layers of mlp_head are nn.Identity so the indices match).
+
+    Per scene the n_b agents are warped to the ego into slots b*L .. b*L+n_b-1 of a zeroed (B*L, H, W, C) map (heal_warp_affine;
+    the padded slots stay zero).  Every pre-norm residual sub-layer is then
+        attention: LayerNorm (heal_mean_layernorm) -> to_qkv 1x1 conv (q rows pre-scaled by dim_head^-0.5 in fp64)
+                   -> heal_swap_attention (window, then grid) -> to_out 1x1 conv + residual
+        FFN:       LayerNorm -> 1x1 conv + bias + GELU -> 1x1 conv + bias + residual
+    and mlp_head is heal_mean_layernorm over all L slots (padded ones included, as the reference's Reduce-mean) -> 1x1 conv.
+    Padded slots are queries (they become non-zero after the first block); only their keys are masked.  The packed weights and
+    the dense relative-position bias are a derived cache, rebuilt when a parameter or the index buffer changes."""
+
+    def __init__(self, args):
+        super().__init__()
+        self.layers = nn.ModuleList([])
+        self.depth = args['depth']
+        input_dim = args['input_dim']
+        mlp_dim = args['mlp_dim']
+        agent_size = args['agent_size']
+        window_size = args['window_size']
+        drop_out = args['drop_out']
+        dim_head = args['dim_head']
+        for _ in range(self.depth):
+            self.layers.append(SwapFusionBlockMask(input_dim, mlp_dim, dim_head, window_size, agent_size, drop_out))
+        self.mlp_head = nn.Sequential(nn.Identity(), nn.Identity(), nn.LayerNorm(input_dim), nn.Linear(input_dim, input_dim),
+                                      nn.Identity())
+        self.input_dim, self.agent_size, self.window_size, self.dim_head = input_dim, agent_size, window_size, dim_head
+        self._derived = None
+
+    def _check(self, C, H, W, L):
+        if L != self.agent_size:
+            raise ValueError(f"CoBEVT: the affine matrix has L = {L} agent slots but agent_size is {self.agent_size}; the "
+                             "reference's relative position bias is sized by agent_size and fails for any other L")
+        if H % self.window_size or W % self.window_size:
+            raise ValueError(f"CoBEVT: the feature map {(H, W)} is not divisible by window_size {self.window_size}; the "
+                             "reference's window rearrange fails for this shape")
+        if C != self.input_dim:
+            raise ValueError(f"CoBEVT: input_dim is {self.input_dim} but the feature map has {C} channels")
+        if self.dim_head != 32:
+            raise NotImplementedError(f"CoBEVT: heal_swap_attention implements dim_head 32 (every shipped config), not {self.dim_head}")
+        if L * self.window_size ** 2 > 128:
+            raise NotImplementedError(f"CoBEVT: heal_swap_attention implements windows of at most 128 tokens, not "
+                                      f"agent_size * window_size^2 = {L * self.window_size ** 2}")
+
+    def _packed(self):
+        sig = engine._sig(*self.modules())
+        if self._derived is None or self._derived[0] != sig:
+            blocks = []
+            for blk in self.layers:
+                parts = []
+                for att, ffd in ((blk.window_attention, blk.window_ffd), (blk.grid_attention, blk.grid_ffd)):
+                    a = att.fn
+                    C = a.to_qkv.in_features
+                    wq = a.to_qkv.weight.detach().double()
+                    wq = torch.cat([wq[:C] * a.scale, wq[C:]]).float()
+                    qkv = _conv_from(wq[:, :, None, None], None, 0)
+                    out = _conv_from(a.to_out[0].weight.detach()[:, :, None, None], None, 0)
+                    # key-major dense bias: bias[h, j, i] = table[index[i, j], h]
+                    bias = a.relative_position_bias_table.weight.detach()[a.relative_position_index]
+                    bias = bias.permute(2, 1, 0).float().contiguous()
+                    l1, l2 = ffd.fn.net[0], ffd.fn.net[3]
+                    f1 = _conv_from(l1.weight.detach()[:, :, None, None], l1.bias.detach(), 0)
+                    f2 = _conv_from(l2.weight.detach()[:, :, None, None], l2.bias.detach(), 0)
+                    parts.append((att.norm, qkv, bias, out, ffd.norm, f1, f2))
+                blocks.append(parts)
+            lin = self.mlp_head[3]
+            head = _conv_from(lin.weight.detach()[:, :, None, None], lin.bias.detach(), 0)
+            self._derived = (sig, blocks, head)
+        return self._derived[1:]
+
+    def forward_nhwc(self, x, record_len, affine_matrix):
+        """x: Act (sumN,H,W,C), affine_matrix (B,L,L,2,3) -> Act (B,H,W,C).  Reads record_len on the host; no other sync."""
+        require_eval(self)
+        rl = _rl(record_len)
+        B, L = affine_matrix.shape[:2]
+        C, H, W = x.C, x.H, x.W
+        self._check(C, H, W, L)
+        if len(rl) != B or any(n < 1 or n > L for n in rl):
+            raise ValueError(f"CoBEVT: record_len {rl} does not fit {B} scenes of at most {L} agents")
+        blocks, head = self._packed()
+        fmt = engine.act_fmt()
+        aff = affine_matrix.to(device=x.device, dtype=torch.float64)
+        X = ops.act_empty(B * L, H, W, C, fmt, x.device)
+        start = 0
+        for b, n in enumerate(rl):
+            ops.warp_affine(x, range(start, start + n), aff[b, 0, :n].contiguous(), out=X.images(b * L, b * L + n))
+            if n < L:
+                X.images(b * L + n, (b + 1) * L).t.zero_()
+            start += n
+        w = self.window_size
+        for parts in blocks:
+            for grid, (norm, qkv, bias, out, fnorm, f1, f2) in enumerate(parts):
+                y = ops.mean_layernorm(X, 1, norm.weight, norm.bias, norm.eps, out_fmt=fmt)
+                a = ops.swap_attention(conv_bn_act(y, qkv), rl, L, w, bool(grid), bias, out_fmt=fmt)
+                X = conv_bn_act(a, out, residual=X)
+                y = ops.mean_layernorm(X, 1, fnorm.weight, fnorm.bias, fnorm.eps, out_fmt=fmt)
+                X = conv_bn_act(conv_bn_act(y, f1, relu=2), f2, residual=X)
+        ln = self.mlp_head[2]
+        y = ops.mean_layernorm(X, L, ln.weight, ln.bias, ln.eps, out_fmt=fmt)
+        return conv_bn_act(y, head)
+
+    def forward(self, x, record_len, affine_matrix):
+        require_eval(self)
+        self._check(x.shape[1], x.shape[2], x.shape[3], affine_matrix.shape[1])
         return ops.act_to_nchw(self.forward_nhwc(ops.to_act(x), record_len, affine_matrix))

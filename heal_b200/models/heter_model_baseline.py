@@ -1,7 +1,7 @@
 """HeterModelBaseline mirror (opencood/models/heter_model_baseline.py:26-236): per-modality encoder ->
 BaseBEVBackbone -> per-agent shrinker -> single-scale fusion -> heads.  Same ctor argument, state-dict keys and forward(data_dict) -> output_dict contract.
-`fusion_method`: att (AttFusion), max (F-Cooper MaxFusion) and v2vnet (V2VNetFusion).  disconet cannot be constructed in the
-reference itself; v2xvit, cobevt, where2comm and who2com are outside the hot-path scope."""
+`fusion_method`: att (AttFusion), max (F-Cooper MaxFusion), v2vnet (V2VNetFusion) and cobevt (CoBEVT).  disconet cannot be
+constructed in the reference itself; v2xvit, where2comm and who2com are outside the hot-path scope."""
 import importlib
 from collections import OrderedDict, Counter
 
@@ -13,7 +13,7 @@ from ..engine import require_eval
 from ..utils.transformation_utils import normalize_pairwise_tfm
 from .sub_modules.base_bev_backbone import BaseBEVBackbone
 from .sub_modules.downsample_conv import DownsampleConv
-from .fuse_modules.fusion_in_one import AttFusion, MaxFusion, V2VNetFusion
+from .fuse_modules.fusion_in_one import AttFusion, CoBEVT, MaxFusion, V2VNetFusion
 from .heter_pyramid_collab import FusedHeads, HeterPyramidCollab
 
 
@@ -58,11 +58,13 @@ class HeterModelBaseline(nn.Module):
             self.fusion_net = MaxFusion()
         elif fm == "v2vnet":
             self.fusion_net = V2VNetFusion(args['v2vnet'])
+        elif fm == "cobevt":
+            self.fusion_net = CoBEVT(args['cobevt'])
         elif fm == "disconet":
             raise NotImplementedError("fusion_method 'disconet': DiscoFusion cannot be constructed in the reference either "
                                       "(it imports opencood.models.fuse_modules.disco_fuse, which the reference does not ship)")
         else:
-            raise NotImplementedError(f"fusion_method '{fm}' is outside the heal_b200 hot-path scope (built: att, max, v2vnet)")
+            raise NotImplementedError(f"fusion_method '{fm}' is outside the heal_b200 hot-path scope (built: att, max, v2vnet, cobevt)")
         self.shrink_flag = 'shrink_header' in args
         if self.shrink_flag:
             self.shrink_conv = DownsampleConv(args['shrink_header'])

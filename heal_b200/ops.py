@@ -771,6 +771,49 @@ def gru_gate(zc: Act, out: Optional[Act] = None, out_fmt: Optional[str] = None) 
     return out
 
 
+def swap_attention(qkv: Act, n_agents: Sequence[int], L: int, window_size: int, grid: bool, bias: torch.Tensor,
+                   out: Optional[Act] = None, out_fmt: Optional[str] = None) -> Act:
+    """CoBEVT window (grid False) or grid (grid True) attention core.  qkv Act (B*L,H,W,3C) = to_qkv output with q pre-scaled;
+    n_agents: host sequence of the B scenes' real-agent counts; bias (C/32, n, n) fp32 device, key-major (bias[h, j, i]),
+    n = L * window_size^2 -> Act (B*L,H,W,C) = softmax over the real agents' keys of (q k^T + bias) v, heads merged."""
+    _need_cuda(bias)
+    B, H, W, C = len(n_agents), qkv.H, qkv.W, qkv.C // 3
+    n = L * window_size * window_size
+    assert qkv.N == B * L and qkv.C == 3 * C and bias.dtype == torch.float32 and bias.is_contiguous()
+    assert bias.shape == (C // 32, n, n)
+    if out is None:
+        out = act_empty(B * L, H, W, C, out_fmt or qkv.fmt, qkv.device)
+    assert (out.N, out.H, out.W, out.C) == (B * L, H, W, C)
+    keys = float(sum(int(v) for v in n_agents)) * window_size * window_size     # valid keys per query, summed over scenes
+    wins = (H // window_size) * (W // window_size)
+    qv, ov = qkv.view(), out.view()
+    with _Prof("swap_attention", 4.0 * keys * C * wins * n,
+               B * L * H * W * float(C) * (3 * BPE[qkv.fmt] + BPE[out.fmt])):
+        rc = lib.heal_swap_attention(ctypes.byref(qv), _host_i32(n_agents), B, L, H, W, C, int(window_size), 1 if grid else 0,
+                                     _p(bias), ctypes.byref(ov), _stream())
+    check(rc, "heal_swap_attention")
+    return out
+
+
+def mean_layernorm(x: Act, n_avg: int, ln_weight: torch.Tensor, ln_bias: torch.Tensor, eps: float,
+                   out: Optional[Act] = None, out_fmt: Optional[str] = None) -> Act:
+    """x Act (N*n_avg,H,W,C) -> Act (N,H,W,C): LayerNorm over channels of the mean of every n_avg consecutive images
+    (n_avg = 1: a plain channels-last LayerNorm)."""
+    _need_cuda(ln_weight, ln_bias)
+    assert x.N % n_avg == 0
+    N, H, W, C = x.N // n_avg, x.H, x.W, x.C
+    if out is None:
+        out = act_empty(N, H, W, C, out_fmt or x.fmt, x.device)
+    assert (out.N, out.H, out.W, out.C) == (N, H, W, C)
+    lw, lb = ln_weight.float().contiguous(), ln_bias.float().contiguous()
+    xv, ov = x.view(), out.view()
+    with _Prof("mean_layernorm", 0, N * H * W * float(C) * (n_avg * BPE[x.fmt] + BPE[out.fmt])):
+        rc = lib.heal_mean_layernorm(ctypes.byref(xv), N, int(n_avg), H, W, C, _p(lw), _p(lb), float(eps), ctypes.byref(ov),
+                                     _stream())
+    check(rc, "heal_mean_layernorm")
+    return out
+
+
 # ------------------------------------------------------------------------------------------------
 # Lift-Splat-Shoot
 # ------------------------------------------------------------------------------------------------

@@ -205,6 +205,24 @@ int heal_v2v_aggregate(const heal_act_t* q, const heal_act_t* p_node, const heal
  * zc = the stacked (update gate | candidate) GRU conv output (npix, 2C). */
 int heal_gru_gate(const heal_act_t* zc, long long npix, int C, const heal_act_t* out, void* stream);
 
+/* CoBEVT window / grid attention core (swap_fusion_modules.py:87-128 with CoBEVT's agent mask, fusion_in_one.py:409-429).
+ * qkv (B*L, H, W, 3C) = the to_qkv 1x1-conv output (q | k | v, head h = channels h*32 .. h*32+31 of each; q already scaled by
+ * 32^-0.5); out (B*L, H, W, C) = the merged heads.  One window has n = L*w*w tokens ordered (agent l, w1, w2):
+ *   grid_mode 0 (window):  window (x, y) = pixels (x*w + w1, y*w + w2)
+ *   grid_mode 1 (grid):    window (x, y) = pixels (w1*H/w + x, w2*W/w + y)
+ * out_i = sum_j softmax_j(q_i . k_j + bias[h][j][i]) v_j over the keys of the n_agents_host[b] real agents of scene b (tokens
+ * j < n_agents_host[b]*w*w); the keys of padded agents are skipped (the reference's -inf), their queries are computed.
+ * bias: (C/32, n, n) fp32 device, KEY-major: bias[h][j][i] = relative_position_bias_table[relative_position_index[i][j]][h].
+ * n_agents_host: HOST array of B counts in [1, L].  C a multiple of 32 (dim_head 32), n <= 128, H and W multiples of w. */
+int heal_swap_attention(const heal_act_t* qkv, const int* n_agents_host, int B, int L, int H, int W, int C,
+                        int window_size, int grid_mode, const float* bias, const heal_act_t* out, void* stream);
+
+/* Mean over n_avg consecutive images, then LayerNorm over the channels (biased variance, eps):
+ * out image o = LayerNorm(mean_{k < n_avg} in image o*n_avg + k) for o < n_out.  n_avg = 1 is a plain LayerNorm.
+ * ln_weight, ln_bias: (C) fp32 device.  C in {64, 128, 192, 256}. */
+int heal_mean_layernorm(const heal_act_t* in, int n_out, int n_avg, int H, int W, int C, const float* ln_weight,
+                        const float* ln_bias, float eps, const heal_act_t* out, void* stream);
+
 /* ---- Lift-Splat-Shoot ------------------------------------------------------------------------
  * heal_lss_cell_index replaces LiftSplatShoot.get_geometry + the index half of voxel_pooling
  * (opencood/models/heter_encoders.py:125-147, :173-185): for every frustum point of every camera image

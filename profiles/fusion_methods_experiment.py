@@ -1,10 +1,11 @@
-"""HeterModelBaseline frames with fusion_method max (lidar_fcooper.yaml) and v2vnet (lidar_v2vnet.yaml), and att at the same
-shapes for comparison: 5 agents, PointPillars on the +-102.4 m range (512^2 pillar grid), BaseBEVBackbone [3,5,8] -> 256^2,
-per-agent shrink header stride 1 (fusion at 256^2) or stride 2 (fusion at 128^2, lidar_v2vnet's conv_gru H/W = 128).
+"""HeterModelBaseline frames with fusion_method max (lidar_fcooper.yaml), v2vnet (lidar_v2vnet.yaml) and cobevt
+(lidar_cobevt.yaml), and att at the same shapes for comparison: 5 agents, PointPillars on the +-102.4 m range (512^2 pillar grid), BaseBEVBackbone [3,5,8] -> 256^2,
+per-agent shrink header stride 1 (fusion at 256^2) or stride 2 (fusion at 128^2: lidar_v2vnet's conv_gru H/W = 128, and
+lidar_cobevt's shape).
 
 Each frame is captured as a CUDA graph (heal_b200.graph.FrameGraph) and replayed after warm-up, timed with CUDA events.  One
 eager frame per model is then run with the `ops._Prof` counters on, and the per-family times are printed.  When the reference
-has been built into oracle/_ref, its own MaxFusion / V2VNetFusion modules are timed eagerly (cuDNN, fp32) on random maps of the
+has been built into oracle/_ref, its own MaxFusion / V2VNetFusion / CoBEVT modules are timed eagerly (cuDNN, fp32) on random maps of the
 same shapes.  Prints the card's name and power limit first; --out DIR writes the records as DIR/fusion_methods.json."""
 import argparse
 import copy
@@ -38,10 +39,22 @@ def model_args(method, shrink_stride):
     elif method == "v2vnet":
         args["v2vnet"] = {"num_iteration": 2, "in_channels": 256, "gru_flag": True, "agg_operator": "avg",
                           "conv_gru": {"H": fused_hw, "W": fused_hw, "num_layers": 1, "kernel_size": [[3, 3]]}}
+    elif method == "cobevt":
+        args["cobevt"] = {"input_dim": 256, "mlp_dim": 256, "agent_size": 5, "window_size": 4, "dim_head": 32, "drop_out": 0.1,
+                          "depth": 3}
     return args
 
 
-CASES = [("fcooper", "max", 1), ("att@256", "att", 1), ("v2vnet", "v2vnet", 2), ("att@128", "att", 2)]
+def load_procedural(m):
+    """Procedural values for every float key (CoBEVT's int64 relative_position_index buffers keep the module's own values)."""
+    from workloads import procedural
+    sd = m.state_dict()
+    sd.update(procedural.make_state_dict({k: v for k, v in procedural.shapes_of(m).items() if sd[k].is_floating_point()}))
+    m.load_state_dict(sd, strict=True)
+    return m
+
+
+CASES = [("fcooper", "max", 1), ("att@256", "att", 1), ("v2vnet", "v2vnet", 2), ("att@128", "att", 2), ("cobevt", "cobevt", 2)]
 
 
 def frame_inputs(n_agents, seed=7):
@@ -56,10 +69,7 @@ def run_case(method, stride, iters, pts, offs, pw, n_agents):
     from heal_b200 import ops
     from heal_b200.graph import FrameGraph
     from heal_b200.models.heter_model_baseline import HeterModelBaseline
-    from workloads import procedural
-    m = HeterModelBaseline(model_args(method, stride)).eval()
-    m.load_state_dict(procedural.make_state_dict(procedural.shapes_of(m)), strict=True)
-    m = m.cuda()
+    m = load_procedural(HeterModelBaseline(model_args(method, stride)).eval()).cuda()
     cap = (pts.shape[0] + 4095) // 4096 * 4096
     fg = FrameGraph(m, n_agents, cap, pw.shape)
     fg.load(pts, offs, pw)
@@ -88,7 +98,7 @@ def reference_fusion_us(iters, n_agents):
     if not os.path.isdir(os.path.join(ROOT, "oracle", "_ref", "opencood")):
         return None
     ref_shim.install()
-    from opencood.models.fuse_modules.fusion_in_one import MaxFusion, V2VNetFusion
+    from opencood.models.fuse_modules.fusion_in_one import CoBEVT, MaxFusion, V2VNetFusion
     from workloads import procedural
     from heal_b200 import synth
     from oracle import nets
@@ -107,6 +117,10 @@ def reference_fusion_us(iters, n_agents):
         x = torch.randn(n_agents, 256, 128, 128, device="cuda")
         v(x, rl, aff)
         out["reference V2VNetFusion @128"] = time_us(lambda: v(x, rl, aff), max(1, iters // 10))
+        del v
+        c = load_procedural(CoBEVT(model_args("cobevt", 2)["cobevt"]).eval()).cuda()
+        c(x, rl, aff)
+        out["reference CoBEVT @128"] = time_us(lambda: c(x, rl, aff), max(1, iters // 10))
     return out
 
 
