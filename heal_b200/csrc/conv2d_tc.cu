@@ -310,11 +310,16 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 #pragma unroll
                 for (int c64 = 0; c64 < BLOCK_N / 64; ++c64) {
                     const int b = stg_count % STG;
+                    // tma_out needs Cout % 64 == 0, so a chunk is wholly inside Cout or wholly past it (the last n-tile of
+                    // Cout = 192, 320, ... against coutp = 256, 384, ...).  A dead chunk reads no bias or residual (both are
+                    // [Cout] / Cout-wide in global memory) but is still staged and stored, clipped by the TMA unit, so the
+                    // buffer rotation and the residual barrier parity stay the same for every chunk.
+                    const bool live = ch0 + 64 * c64 < p.Cout;
                     // the chunk's bias pairs, requested before the waits (the shared-memory stores below are compiler barriers)
                     float2 bb[8];
 #pragma unroll
                     for (int jj = 0; jj < 8; ++jj)
-                        bb[jj] = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + ch0 + 64 * c64 + 8 * jj + fcol)) : make_float2(0.f, 0.f);
+                        bb[jj] = (p.bias && live) ? __ldg(reinterpret_cast<const float2*>(p.bias + ch0 + 64 * c64 + 8 * jj + fcol)) : make_float2(0.f, 0.f);
                     if (res_tma) {
                         // (A') the store that last used buffer (i+1) % STG has been read out -> request residual(i+1) into it, then wait
                         // for residual(i) in buffer b (STG == 3: a full chunk of lead; STG == 2: the lead is the chunk minus the store drain)
@@ -350,7 +355,7 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 #pragma unroll
                                 for (int h = 0; h < 2; ++h) { v[2 * h] += bf16_lo_f(rs[2 + h]); v[2 * h + 1] += bf16_hi_f(rs[2 + h]); }
                             }
-                        } else if (p.res_f32 && !(p.dbg & 8)) {
+                        } else if (p.res_f32 && live && !(p.dbg & 8)) {
 #pragma unroll
                             for (int h = 0; h < 2; ++h) {
                                 if (valid[h]) {
