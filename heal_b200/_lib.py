@@ -52,6 +52,11 @@ SIGNATURES = {
     "heal_gru_gate": (_i, [_ap, _c.c_longlong, _i, _ap, _vp]),
     "heal_swap_attention": (_i, [_ap, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _ap, _vp]),
     "heal_mean_layernorm": (_i, [_ap, _i, _i, _i, _i, _i, _vp, _vp, _c.c_float, _ap, _vp]),
+    "heal_window_attention": (_i, [_ap, _i, _i, _i, _i, _i, _i, _vp, _ap, _vp]),
+    "heal_cav_attention": (_i, [_ap, _vp, _i, _i, _i, _i, _i, _ap, _vp]),
+    "heal_split_attn_workspace": (_sz, [_i, _i]),
+    "heal_split_attn": (_i, [_ap, _ap, _i, _i, _i, _i, _vp, _vp, _vp, _c.c_float, _vp, _vp, _sz, _ap, _vp]),
+    "heal_sttf_resample": (_i, [_ap, _vp, _i, _i, _i, _i, _ap, _vp]),
     "heal_act_convert": (_i, [_ap, _ap, _sz, _i, _vp]),
     "heal_postprocess_workspace": (_sz, [_i, _i, _i, _i]),
     "heal_box_decode_nms": (_i, [_ap, _ap, _ap, _vp, _i, _i, _i, _c.c_float, _c.c_float, _i, _vp, _i, _c.c_float, _i,

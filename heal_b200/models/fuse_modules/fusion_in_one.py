@@ -1,7 +1,8 @@
 """Fusion operator mirrors of opencood/models/fuse_modules/fusion_in_one.py: AttFusion (:126-151), MaxFusion (:87-124),
-V2VNetFusion (:203-318) and CoBEVT (:374-429), with the reference's `forward(x, record_len, affine_matrix)` signature (NCHW) and
-`forward_nhwc` (conv-engine activations).  DiscoFusion cannot be constructed in the reference (it imports a `disco_fuse` module
-the reference does not ship); V2X-ViT, Where2comm and Who2com are out of scope (SURVEY.md 2.1 row 14)."""
+V2VNetFusion (:203-318), V2XViTFusion (:320-372) and CoBEVT (:374-429), with the reference's `forward(x, record_len,
+affine_matrix)` signature (NCHW) and `forward_nhwc` (conv-engine activations).  DiscoFusion cannot be constructed in the
+reference (it imports a `disco_fuse` module the reference does not ship); Where2comm and Who2com are out of scope (SURVEY.md 2.1
+row 14)."""
 import numpy as np
 import torch
 import torch.nn as nn
@@ -318,6 +319,158 @@ class CoBEVT(nn.Module):
         ln = self.mlp_head[2]
         y = ops.mean_layernorm(X, L, ln.weight, ln.bias, ln.eps, out_fmt=fmt)
         return conv_bn_act(y, head)
+
+    def forward(self, x, record_len, affine_matrix):
+        require_eval(self)
+        self._check(x.shape[1], x.shape[2], x.shape[3], affine_matrix.shape[1])
+        return ops.act_to_nchw(self.forward_nhwc(ops.to_act(x), record_len, affine_matrix))
+
+
+_V2XVIT_SCOPE = "outside the heal_b200 hot-path scope"
+
+
+class V2XViTFusion(nn.Module):
+    """V2X-ViT (fusion_in_one.py:320-372) with the reference's ctor and state-dict keys (`fusion_net.encoder.layers.{i}.0.layers.0.
+    {0,1}` the HGT and pyramid-window PreNorms, `.{i}.1` the FFN PreNorm, `fusion_net.encoder.prior_feed`).
+
+    The GPU path keeps only what reaches the ego output of the reference:
+      - the n_b real agents of each scene, not L padded slots: padded agents are masked as keys of the agent attention and every
+        other step is per agent, so they never reach a real one.  Images are ordered egos first, then each scene's others;
+      - agent types are always 0 (V2XViTFusion feeds a zero prior encoding), so HGTCavAttention is multi-head attention with
+        relation_att[0] and dim_head^-0.5 folded into the q rows and relation_msg[0] into the v rows of one to_qkv 1x1 conv
+        (fp64 folding); the ROI mask is all ones for the identity correction, so the key mask is the agent mask;
+      - only slot 0 is read after the last agent attention, so the last layer's agent attention has ego queries only and its
+        window attention, SplitAttn and FFN run on the egos.
+    Per scene the agents are warped to the ego (heal_warp_affine), the others resampled by the STTF matrix (heal_sttf_resample).
+    Each layer: LayerNorm -> to_qkv conv -> heal_cav_attention -> a_linears[0] conv + residual; LayerNorm -> the three branch
+    to_qkv as one conv -> heal_window_attention per branch -> the three to_out convs -> heal_split_attn (+ residual);
+    LayerNorm -> conv + GELU -> conv + residual.  The folded weights, dense biases and STTF matrices are a derived cache."""
+
+    def __init__(self, args):
+        super().__init__()
+        from ..sub_modules.v2xvit_basic import V2XTransformer
+        enc = args['transformer']['encoder']
+        cav, pw = enc['cav_att_config'], enc['pwindow_att_config']
+        if enc.get('use_RTE') or cav.get('use_RTE'):
+            raise NotImplementedError(f"V2XViTFusion: use_RTE is {_V2XVIT_SCOPE} (no shipped config enables it)")
+        if not cav['use_hetero']:
+            raise NotImplementedError(f"V2XViTFusion: use_hetero false (CavAttention) is {_V2XVIT_SCOPE}")
+        if pw['fusion_method'] != 'split_attn':
+            raise NotImplementedError(f"V2XViTFusion: window fusion '{pw['fusion_method']}' is {_V2XVIT_SCOPE} (built: split_attn)")
+        if pw['dim'] != 256 or cav['dim'] != 256:
+            raise ValueError(f"V2XViTFusion: split_attn is SplitAttn(256) in the reference and needs dim 256, not "
+                             f"{cav['dim']} / {pw['dim']}")
+        if len(pw['window_size']) != 3:
+            raise ValueError("V2XViTFusion: split_attn fuses exactly 3 window branches (the reference asserts it)")
+        if cav['dim_head'] != 32:
+            raise NotImplementedError(f"V2XViTFusion: heal_cav_attention implements dim_head 32, not {cav['dim_head']}")
+        for ws, dh in zip(pw['window_size'], pw['dim_head']):
+            if ws not in (4, 8, 16) or dh not in (16, 32, 64):
+                raise NotImplementedError(f"V2XViTFusion: heal_window_attention implements windows 4/8/16 and dim_head "
+                                          f"16/32/64, not window {ws} with dim_head {dh}")
+        self.fusion_net = V2XTransformer(args['transformer'])
+        self.dim = cav['dim']
+        self.window_sizes = list(pw['window_size'])
+        self._derived = None
+
+    def _check(self, C, H, W, L):
+        if C != self.dim:
+            raise ValueError(f"V2XViTFusion: dim is {self.dim} but the feature map has {C} channels")
+        for ws in self.window_sizes:
+            if H % ws or W % ws:
+                raise ValueError(f"V2XViTFusion: the feature map {(H, W)} is not divisible by window size {ws}; the "
+                                 "reference's window rearrange fails for this shape")
+        if L > 8:
+            raise NotImplementedError(f"V2XViTFusion: heal_cav_attention implements at most 8 agents, not L = {L}")
+
+    def _packed(self, H, W, device):
+        sig = engine._sig(*self.modules())
+        if self._derived is None or self._derived[0] != sig:
+            layers = []
+            for blk, ffn in self.fusion_net.encoder.layers:
+                cav_pre, win_pre = blk.layers[0]
+                a = cav_pre.fn
+                dh, hd = a.dim_head, a.heads
+                q, k, v = a.q_linears[0], a.k_linears[0], a.v_linears[0]
+                ra = a.relation_att.detach()[0].double()                        # (heads, p, q)
+                rm = a.relation_msg.detach()[0].double()
+                wq = q.weight.detach().double().reshape(hd, dh, -1)
+                bq = q.bias.detach().double().reshape(hd, dh)
+                wv = v.weight.detach().double().reshape(hd, dh, -1)
+                bv = v.bias.detach().double().reshape(hd, dh)
+                # q'_m = scale * R_att[m]^T q_m, v'_m = R_msg[m]^T v_m
+                wq2 = torch.einsum("mpq,mpc->mqc", ra, wq).reshape(hd * dh, -1) * a.scale
+                bq2 = torch.einsum("mpq,mp->mq", ra, bq).reshape(-1) * a.scale
+                wv2 = torch.einsum("mpc,mpk->mck", rm, wv).reshape(hd * dh, -1)
+                bv2 = torch.einsum("mpc,mp->mc", rm, bv).reshape(-1)
+                w = torch.cat([wq2, k.weight.detach().double(), wv2]).float()
+                b = torch.cat([bq2, k.bias.detach().double(), bv2]).float()
+                hgt_qkv = _conv_from(w[:, :, None, None], b, 0)
+                al = a.a_linears[0]
+                hgt_out = _conv_from(al.weight.detach()[:, :, None, None], al.bias.detach(), 0)
+                pwa = win_pre.fn
+                wq3, branches, outs = [], [], []
+                for br in pwa.pwmsa:
+                    inner = br.heads * br.dim_head
+                    wt = br.to_qkv.weight.detach().double()
+                    wq3.append(torch.cat([wt[:inner] * br.scale, wt[inner:]]))
+                    branches.append((br.heads, br.dim_head, br.window_size, br.dense_bias().float().contiguous()))
+                    lo = br.to_out[0]
+                    outs.append(_conv_from(lo.weight.detach()[:, :, None, None], lo.bias.detach(), 0))
+                win_qkv = _conv_from(torch.cat(wq3).float()[:, :, None, None], None, 0)
+                sa = pwa.split_attn
+                gate = (sa.fc1.weight.detach().float().t().contiguous(), sa.bn1, sa.fc2.weight.detach().float().t().contiguous())
+                l1, l2 = ffn.fn.net[0], ffn.fn.net[3]
+                f1 = _conv_from(l1.weight.detach()[:, :, None, None], l1.bias.detach(), 0)
+                f2 = _conv_from(l2.weight.detach()[:, :, None, None], l2.bias.detach(), 0)
+                layers.append((cav_pre.norm, hgt_qkv, hgt_out, win_pre.norm, win_qkv, branches, outs, gate, ffn.norm, f1, f2))
+            self._derived = (sig, layers, {})
+        thetas = self._derived[2]
+        key = (H, W, str(device))
+        if key not in thetas:
+            thetas[key] = self.fusion_net.encoder.sttf.theta(H, W).to(device)
+        return self._derived[1], thetas[key]
+
+    def forward_nhwc(self, x, record_len, affine_matrix):
+        """x: Act (sumN,H,W,C), affine_matrix (B,L,L,2,3) -> Act (B,H,W,C), the ego slot.  Reads record_len on the host; no
+        other sync."""
+        require_eval(self)
+        rl = _rl(record_len)
+        B, L = affine_matrix.shape[:2]
+        C, H, W = x.C, x.H, x.W
+        self._check(C, H, W, L)
+        if len(rl) != B or any(n < 1 or n > L for n in rl) or sum(rl) != x.N:
+            raise ValueError(f"V2XViTFusion: record_len {rl} does not fit {B} scenes of at most {L} agents and {x.N} maps")
+        layers, theta = self._packed(H, W, x.device)
+        fmt = engine.act_fmt()
+        aff = affine_matrix.to(device=x.device, dtype=torch.float64)
+        N = sum(rl)
+        starts = [sum(rl[:b]) for b in range(B)]
+        X = ops.act_empty(N, H, W, C, fmt, x.device)
+        ops.warp_affine(x, starts, aff[:, 0, 0].contiguous(), out=X.images(0, B))
+        if N > B:
+            src = [starts[b] + j for b in range(B) for j in range(1, rl[b])]
+            th = torch.cat([aff[b, 0, 1:rl[b]] for b in range(B) if rl[b] > 1])
+            warped = ops.warp_affine(x, src, th, out_fmt=fmt)
+            ops.sttf_resample(warped, theta.expand(N - B, 2, 3).contiguous(), out=X.images(B, N))
+        for i, (n1, hgt_qkv, hgt_out, n2, win_qkv, branches, outs, gate, n3, f1, f2) in enumerate(layers):
+            last = i == len(layers) - 1
+            y = ops.mean_layernorm(X, 1, n1.weight, n1.bias, n1.eps, out_fmt=fmt)
+            a = ops.cav_attention(conv_bn_act(y, hgt_qkv), rl, ego_only=last, out_fmt=fmt)
+            X = conv_bn_act(a, hgt_out, residual=X.images(0, B) if last else X)
+            y = ops.mean_layernorm(X, 1, n2.weight, n2.bias, n2.eps, out_fmt=fmt)
+            qkv = conv_bn_act(y, win_qkv)
+            o = ops.act_empty(X.N, H, W, 3 * C, fmt, x.device)
+            off = 0
+            for k, ((heads, dh, ws, bias), out_conv) in enumerate(zip(branches, outs)):
+                att = ops.window_attention(qkv, heads, dh, ws, bias, qkv_coffset=off, out_fmt=fmt)
+                conv_bn_act(att, out_conv, out=o, out_coffset=k * C)
+                off += 3 * heads * dh
+            fc1_t, ln, fc2_t = gate
+            X = ops.split_attn(o, X, fc1_t, ln.weight, ln.bias, ln.eps, fc2_t, out_fmt=fmt)
+            y = ops.mean_layernorm(X, 1, n3.weight, n3.bias, n3.eps, out_fmt=fmt)
+            X = conv_bn_act(conv_bn_act(y, f1, relu=2), f2, residual=X)
+        return X
 
     def forward(self, x, record_len, affine_matrix):
         require_eval(self)

@@ -1,7 +1,7 @@
 """HeterModelBaseline mirror (opencood/models/heter_model_baseline.py:26-236): per-modality encoder ->
 BaseBEVBackbone -> per-agent shrinker -> single-scale fusion -> heads.  Same ctor argument, state-dict keys and forward(data_dict) -> output_dict contract.
-`fusion_method`: att (AttFusion), max (F-Cooper MaxFusion), v2vnet (V2VNetFusion) and cobevt (CoBEVT).  disconet cannot be
-constructed in the reference itself; v2xvit, where2comm and who2com are outside the hot-path scope."""
+`fusion_method`: att (AttFusion), max (F-Cooper MaxFusion), v2vnet (V2VNetFusion), v2xvit (V2XViTFusion) and cobevt (CoBEVT).
+disconet cannot be constructed in the reference itself; where2comm and who2com are outside the hot-path scope."""
 import importlib
 from collections import OrderedDict, Counter
 
@@ -13,7 +13,7 @@ from ..engine import require_eval
 from ..utils.transformation_utils import normalize_pairwise_tfm
 from .sub_modules.base_bev_backbone import BaseBEVBackbone
 from .sub_modules.downsample_conv import DownsampleConv
-from .fuse_modules.fusion_in_one import AttFusion, CoBEVT, MaxFusion, V2VNetFusion
+from .fuse_modules.fusion_in_one import AttFusion, CoBEVT, MaxFusion, V2VNetFusion, V2XViTFusion
 from .heter_pyramid_collab import FusedHeads, HeterPyramidCollab
 
 
@@ -60,11 +60,16 @@ class HeterModelBaseline(nn.Module):
             self.fusion_net = V2VNetFusion(args['v2vnet'])
         elif fm == "cobevt":
             self.fusion_net = CoBEVT(args['cobevt'])
+        elif fm == "v2xvit":
+            if 'v2xvit' not in args:
+                raise NotImplementedError("fusion_method 'v2xvit' without a `v2xvit:` block is outside the heal_b200 hot-path "
+                                          "scope (no shipped config omits it)")
+            self.fusion_net = V2XViTFusion(args['v2xvit'])
         elif fm == "disconet":
             raise NotImplementedError("fusion_method 'disconet': DiscoFusion cannot be constructed in the reference either "
                                       "(it imports opencood.models.fuse_modules.disco_fuse, which the reference does not ship)")
         else:
-            raise NotImplementedError(f"fusion_method '{fm}' is outside the heal_b200 hot-path scope (built: att, max, v2vnet, cobevt)")
+            raise NotImplementedError(f"fusion_method '{fm}' is outside the heal_b200 hot-path scope (built: att, max, v2vnet, v2xvit, cobevt)")
         self.shrink_flag = 'shrink_header' in args
         if self.shrink_flag:
             self.shrink_conv = DownsampleConv(args['shrink_header'])

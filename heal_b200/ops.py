@@ -814,6 +814,89 @@ def mean_layernorm(x: Act, n_avg: int, ln_weight: torch.Tensor, ln_bias: torch.T
     return out
 
 
+def window_attention(qkv: Act, heads: int, dim_head: int, window_size: int, bias: torch.Tensor, qkv_coffset: int = 0,
+                     out: Optional[Act] = None, out_coffset: int = 0, out_fmt: Optional[str] = None) -> Act:
+    """One V2X-ViT window-attention branch.  qkv Act (N,H,W,>=3*heads*dim_head): q | k | v of the branch from channel
+    qkv_coffset (q pre-scaled); bias (w^2, w^2) fp32 device, query-major -> Act (N,H,W,heads*dim_head), or written to
+    channels out_coffset .. of `out`: softmax(q k^T + bias) v per window and head, heads merged."""
+    _need_cuda(bias)
+    N, H, W = qkv.N, qkv.H, qkv.W
+    inner, n = heads * dim_head, window_size * window_size
+    assert qkv_coffset + 3 * inner <= qkv.C and bias.dtype == torch.float32 and bias.is_contiguous() and bias.shape == (n, n)
+    if out is None:
+        out = act_empty(N, H, W, inner, out_fmt or qkv.fmt, qkv.device)
+    assert (out.N, out.H, out.W) == (N, H, W) and out_coffset + inner <= out.C
+    qv, ov = qkv.view(qkv_coffset), out.view(out_coffset)
+    with _Prof("window_attention", 4.0 * N * H * W * n * inner,
+               N * H * W * float(inner) * (3 * BPE[qkv.fmt] + BPE[out.fmt])):
+        rc = lib.heal_window_attention(ctypes.byref(qv), N, H, W, int(heads), int(dim_head), int(window_size), _p(bias),
+                                       ctypes.byref(ov), _stream())
+    check(rc, "heal_window_attention")
+    return out
+
+
+def cav_attention(qkv: Act, n_agents: Sequence[int], ego_only: bool, out: Optional[Act] = None,
+                  out_fmt: Optional[str] = None) -> Act:
+    """V2X-ViT per-pixel agent attention (HGTCavAttention with agent types 0).  qkv Act (N,H,W,3C), N = sum(n_agents), images
+    ordered egos first (image b = ego of scene b), then each scene's other agents in scene order -> Act (N,H,W,C), or
+    (B,H,W,C) for the egos only: softmax over the scene's agents of q_i . k_j, then sum_j p_j v_j, per head of 32."""
+    B, H, W, C = len(n_agents), qkv.H, qkv.W, qkv.C // 3
+    total = sum(int(v) for v in n_agents)
+    assert qkv.N == total and qkv.C == 3 * C
+    nq = B if ego_only else total
+    if out is None:
+        out = act_empty(nq, H, W, C, out_fmt or qkv.fmt, qkv.device)
+    assert (out.N, out.H, out.W, out.C) == (nq, H, W, C)
+    pairs = float(sum(int(v) for v in n_agents)) if ego_only else float(sum(int(v) ** 2 for v in n_agents))
+    qv, ov = qkv.view(), out.view()
+    with _Prof("cav_attention", 4.0 * pairs * H * W * C, H * W * float(C) * (2 * total + nq) * BPE[qkv.fmt]
+               + nq * H * W * float(C) * BPE[out.fmt]):
+        rc = lib.heal_cav_attention(ctypes.byref(qv), _host_i32(n_agents), B, H, W, C, 1 if ego_only else 0,
+                                    ctypes.byref(ov), _stream())
+    check(rc, "heal_cav_attention")
+    return out
+
+
+def split_attn(o: Act, x: Act, fc1_t: torch.Tensor, ln_weight: torch.Tensor, ln_bias: torch.Tensor, eps: float,
+               fc2_t: torch.Tensor, out: Optional[Act] = None, out_fmt: Optional[str] = None) -> Act:
+    """SplitAttn + residual.  o Act (N,H,W,3C) = the three branch outputs side by side, x Act (N,H,W,C) -> Act (N,H,W,C) =
+    sum_r o_r * gate_r + x, gate = the per-image softmax gate of split_attn.py (fc1_t (C,C), fc2_t (C,3C): transposed Linear
+    weights, fp32 device)."""
+    _need_cuda(fc1_t, fc2_t, ln_weight, ln_bias)
+    N, H, W, C = x.N, x.H, x.W, x.C
+    assert (o.N, o.H, o.W, o.C) == (N, H, W, 3 * C)
+    assert fc1_t.shape == (C, C) and fc2_t.shape == (C, 3 * C) and fc1_t.is_contiguous() and fc2_t.is_contiguous()
+    if out is None:
+        out = act_empty(N, H, W, C, out_fmt or x.fmt, x.device)
+    assert (out.N, out.H, out.W, out.C) == (N, H, W, C)
+    lw, lb = ln_weight.float().contiguous(), ln_bias.float().contiguous()
+    nbytes = int(lib.heal_split_attn_workspace(N, C))
+    ws = _workspace(x.device, nbytes)
+    ov, xv, dv = o.view(), x.view(), out.view()
+    with _Prof("split_attn", N * (2.0 * C * C * 4 + 6.0 * H * W * C),
+               N * H * W * float(C) * (6 * BPE[o.fmt] + BPE[x.fmt] + BPE[out.fmt])):
+        rc = lib.heal_split_attn(ctypes.byref(ov), ctypes.byref(xv), N, H, W, C, _p(fc1_t), _p(lw), _p(lb), float(eps),
+                                 _p(fc2_t), _p(ws), ws.numel(), ctypes.byref(dv), _stream())
+    check(rc, "heal_split_attn")
+    return out
+
+
+def sttf_resample(src: Act, theta: torch.Tensor, out: Optional[Act] = None, out_fmt: Optional[str] = None) -> Act:
+    """V2X-ViT STTF warp: out image k = grid_sample(src image k, affine_grid(theta[k])), bilinear, zeros, align_corners=True.
+    theta (N,2,3) fp32 on the device."""
+    _need_cuda(theta)
+    N, H, W, C = src.N, src.H, src.W, src.C
+    assert theta.dtype == torch.float32 and theta.is_contiguous() and theta.shape == (N, 2, 3)
+    if out is None:
+        out = act_empty(N, H, W, C, out_fmt or src.fmt, src.device)
+    assert (out.N, out.H, out.W, out.C) == (N, H, W, C)
+    sv, ov = src.view(), out.view()
+    with _Prof("sttf_resample", 8.0 * N * C * H * W, N * (BPE[src.fmt] + BPE[out.fmt]) * float(C) * H * W):
+        rc = lib.heal_sttf_resample(ctypes.byref(sv), _p(theta), N, H, W, C, ctypes.byref(ov), _stream())
+    check(rc, "heal_sttf_resample")
+    return out
+
+
 # ------------------------------------------------------------------------------------------------
 # Lift-Splat-Shoot
 # ------------------------------------------------------------------------------------------------

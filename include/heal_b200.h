@@ -223,6 +223,43 @@ int heal_swap_attention(const heal_act_t* qkv, const int* n_agents_host, int B, 
 int heal_mean_layernorm(const heal_act_t* in, int n_out, int n_avg, int H, int W, int C, const float* ln_weight,
                         const float* ln_bias, float eps, const heal_act_t* out, void* stream);
 
+/* ---- V2X-ViT (fusion_in_one.py:320-372, sub_modules/v2xvit_basic.py) ---------------------------
+ * One BaseWindowAttention branch (mswin.py:20-92): softmax(q k^T + bias) v over the w x w windows of every image, on the
+ * tensor cores.  qkv (n_img, H, W, 3*heads*dim_head) = the branch's to_qkv 1x1-conv output from the view's coffset
+ * (q | k | v, head m = channels m*dim_head .. of each; q already scaled by dim_head^-0.5); out (n_img, H, W, heads*dim_head)
+ * = the merged heads, at the view's coffset (a channel slice of a wider map is fine).  Window (x, y) holds pixels
+ * (x*w + w1, y*w + w2), token t = w1*w + w2.  bias: (w^2, w^2) fp32 device, query-major, shared by every head and window.
+ * bf16 storage: bf16 operands, fp32 accumulation; fp32 and split-bf16 storage: split-bf16 products (fp32-equivalent).
+ * window_size in {4, 8, 16}, dim_head in {16, 32, 64}, H and W multiples of window_size; bias 8-byte aligned, data pointers,
+ * channel offsets and strides of qkv / out even (pairs of channels are read and written together). */
+int heal_window_attention(const heal_act_t* qkv, int n_img, int H, int W, int heads, int dim_head, int window_size,
+                          const float* bias, const heal_act_t* out, void* stream);
+
+/* The per-pixel HGTCavAttention core (hmsa.py) with every agent of type 0: for each query agent i, head and pixel,
+ * softmax_j(q_i . k_j) over the n_b real agents of its scene, then sum_j p_j v_j.  qkv (N, H, W, 3C) = q | k | v of the
+ * folded to_qkv conv (relation_att[0] and dim_head^-0.5 folded into q, relation_msg[0] into v), dim_head 32.  Image layout:
+ * the ego of scene b is image b (b < B); its other n_b - 1 agents follow at image B + sum_{b' < b} (n_b' - 1).  ego_only 0:
+ * out has the N images of qkv; ego_only 1: out (B, H, W, C) holds the egos' outputs only.  n_agents_host: HOST array of B
+ * counts in [1, 8], all checked before anything is launched. */
+int heal_cav_attention(const heal_act_t* qkv, const int* n_agents_host, int B, int H, int W, int C, int ego_only,
+                       const heal_act_t* out, void* stream);
+
+/* SplitAttn (split_attn.py) with the PreNorm residual: o (n_img, H, W, 3C) = the three to_out outputs side by side, x the
+ * residual.  gate = softmax over the 3 branches of fc2(ReLU(LayerNorm(fc1(mean_{H,W}(o_0 + o_1 + o_2))))) per image and
+ * channel; out = o_0 * g_0 + o_1 * g_1 + o_2 * g_2 + x (out may be x).  fc1_t (C, C) and fc2_t (C, 3C) fp32 device, the
+ * Linear weights transposed (fc1_t[k][c] = fc1.weight[c][k]).  The pooled sum is reduced in a fixed order (no atomics).
+ * C = 256.  workspace: heal_split_attn_workspace(n_img, C) bytes of device memory, 16-byte aligned. */
+size_t heal_split_attn_workspace(int n_img, int C);
+int heal_split_attn(const heal_act_t* o, const heal_act_t* x, int n_img, int H, int W, int C, const float* fc1_t,
+                    const float* ln_w, const float* ln_b, float eps, const float* fc2_t, void* workspace, size_t ws_bytes,
+                    const heal_act_t* out, void* stream);
+
+/* The STTF resample (v2xvit_basic.py:12-33, torch_transformation_utils.warp_affine): out image k = F.grid_sample(src image k,
+ * F.affine_grid(theta[k], align_corners=True)), bilinear, zeros padding, align_corners=True.  theta: (n_img, 2, 3) fp32
+ * device.  C a multiple of 4. */
+int heal_sttf_resample(const heal_act_t* src, const float* theta, int n_img, int H, int W, int C, const heal_act_t* out,
+                       void* stream);
+
 /* ---- Lift-Splat-Shoot ------------------------------------------------------------------------
  * heal_lss_cell_index replaces LiftSplatShoot.get_geometry + the index half of voxel_pooling
  * (opencood/models/heter_encoders.py:125-147, :173-185): for every frustum point of every camera image
