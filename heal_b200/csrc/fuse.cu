@@ -516,6 +516,19 @@ static inline ActV to_view(const heal_act_t* a) {
     return v;
 }
 
+// Views read / written 4 channels at a time (act_load4 / act_store4): every 4-channel group must start 16 B-aligned in fp32
+// and 8 B-aligned in each bf16 plane, so the base pointer as well as the channel stride, offset and plane stride.
+static inline bool aligned4(const heal_act_t* a) {
+    const uintptr_t need = a->fmt == 0 ? 15 : 7;
+    return ((uintptr_t)a->data & need) == 0 && (a->cstride & 3) == 0 && (a->coffset & 3) == 0 &&
+           (a->fmt == 0 || (a->plane_stride & 3) == 0);
+}
+// The 8-channel split kernels load 16 B per plane: a 16 B-aligned base and channel groups of 8.
+static inline bool aligned8_split(const heal_act_t* a) {
+    return a->fmt == 2 && ((uintptr_t)a->data & 15) == 0 && (a->cstride & 7) == 0 && (a->coffset & 7) == 0 &&
+           (a->plane_stride & 7) == 0;
+}
+
 extern "C" int heal_pyramid_fuse_level(const heal_act_t* feat, const float* occ, const double* theta,
                                        const int* crop_windows, int n_agents, int H, int W, int C, int align_corners,
                                        const long long* agent_feat_offsets_host, const long long* agent_occ_offsets_host,
@@ -524,7 +537,7 @@ extern "C" int heal_pyramid_fuse_level(const heal_act_t* feat, const float* occ,
     if (n_agents < 1 || n_agents > MAX_AGENTS) return HEAL_ERR_UNSUPPORTED;
     if (rows <= 0) { row0 = 0; rows = H; }
     if (row0 < 0 || row0 + rows > H) return HEAL_ERR_ARG;
-    if ((C & 3) || (feat->cstride & 3) || (feat->coffset & 3) || (out->cstride & 3) || (out->coffset & 3)) return HEAL_ERR_UNSUPPORTED;
+    if ((C & 3) || !aligned4(feat) || !aligned4(out)) return HEAL_ERR_UNSUPPORTED;
     FuseP p;
     p.feat = to_view(feat); p.occ = occ; p.theta = theta; p.crop = crop_windows; p.out = to_view(out);
     p.n = n_agents; p.H = H; p.W = W; p.C = C; p.align = align_corners;
@@ -538,9 +551,9 @@ extern "C" int heal_pyramid_fuse_level(const heal_act_t* feat, const float* occ,
     }
     cudaStream_t st = (cudaStream_t)stream_;
     const int HW = rows * W;
-    // split-bf16 input, 16 B-aligned channel groups, per-agent element indices that fit 31 bits: the 8-channel kernel
-    if (feat->fmt == 2 && (C & 7) == 0 && (feat->cstride & 7) == 0 && (feat->coffset & 7) == 0 && (feat->plane_stride & 7) == 0 && off8 &&
-        (long long)H * W * feat->cstride < (1LL << 31)) {
+    // split-bf16 input, 16 B-aligned channel groups (base pointer included), per-agent element indices that fit 31 bits:
+    // the 8-channel kernel; any other view takes the generic one
+    if (aligned8_split(feat) && (C & 7) == 0 && off8 && (long long)H * W * feat->cstride < (1LL << 31)) {
         if (C >= 256)      k_pyramid_fuse_split8<8><<<(HW + 7) / 8, 256, 0, st>>>(p);
         else if (C >= 128) k_pyramid_fuse_split8<16><<<(HW + 15) / 16, 256, 0, st>>>(p);
         else               k_pyramid_fuse_split8<32><<<(HW + 31) / 32, 256, 0, st>>>(p);
@@ -557,12 +570,12 @@ extern "C" int heal_att_fuse(const heal_act_t* feat, const double* theta, int n_
                              const heal_act_t* out, void* stream_) {
     if (!feat || !feat->data || !theta || !out || !out->data) return HEAL_ERR_ARG;
     if (n_agents < 1 || n_agents > MAX_AGENTS) return HEAL_ERR_UNSUPPORTED;
-    if ((C % 128) || C > 512 || (feat->cstride & 3) || (feat->coffset & 3) || (out->cstride & 3) || (out->coffset & 3)) return HEAL_ERR_UNSUPPORTED;
+    if ((C % 128) || C > 512 || !aligned4(feat) || !aligned4(out)) return HEAL_ERR_UNSUPPORTED;
     AttP p;
     p.feat = to_view(feat); p.theta = theta; p.out = to_view(out); p.n = n_agents; p.H = H; p.W = W; p.C = C; p.align = 0;
     p.inv_sqrt_dim = 1.0f / sqrtf((float)C);
     cudaStream_t st = (cudaStream_t)stream_;
-    if (feat->fmt == 2 && C <= 256 && (C & 7) == 0 && (feat->cstride & 7) == 0 && (feat->coffset & 7) == 0 && (feat->plane_stride & 7) == 0) {
+    if (aligned8_split(feat) && C <= 256) {
         if (n_agents <= 5) k_att_fuse_split8<5><<<(H * W + 3) / 4, 128, 0, st>>>(p);       // register file sized for the scene
         else k_att_fuse_split8<MAX_AGENTS><<<(H * W + 3) / 4, 128, 0, st>>>(p);
         return heal_check_launch();
@@ -577,10 +590,6 @@ extern "C" int heal_att_fuse(const heal_act_t* feat, const double* theta, int n_
     return heal_check_launch();
 }
 
-// views read / written 4 channels at a time: 16 B-aligned fp32, 8 B-aligned bf16 planes
-static inline bool aligned4(const heal_act_t* a) {
-    return (a->cstride & 3) == 0 && (a->coffset & 3) == 0 && (a->fmt == 0 || (a->plane_stride & 3) == 0);
-}
 static inline long long grid_x(int H, int W, int C) { return ((long long)H * W * (C / 4) + 255) / 256; }
 
 extern "C" int heal_max_fuse(const heal_act_t* feat, const double* theta, int n_agents, int H, int W, int C,

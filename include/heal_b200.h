@@ -169,25 +169,34 @@ int heal_bottleneck_tc(const void* x, size_t x_plane_stride, int N, int H, int W
  *     (j*H*W*cstride, j*H*W).  This is how the kernel reads the agents straight out of the all-gathered buffer of the
  *     agent-per-GPU partition (SURVEY.md 8e) without an unpack copy.
  *   row0, rows: produce output rows [row0, row0+rows) only (row-sharded fusion tail); rows <= 0 = the whole map
- *   out (rows,W,C): the output slab, its pixel 0 is (row0, 0) */
+ *   out (rows,W,C): the output slab, its pixel 0 is (row0, 0)
+ * Alignment: C, the channel strides and offsets of feat and out, their plane strides and the agent feature offsets are
+ * multiples of 4 elements, and feat->data / out->data are 16-byte aligned for fp32 and 8-byte aligned for bf16 / split;
+ * anything else returns HEAL_ERR_UNSUPPORTED.  Split input takes the 8-channel kernel only when C, its strides, offsets and
+ * agent offsets are multiples of 8 and feat->data is 16-byte aligned, the generic kernel otherwise (same results). */
 int heal_pyramid_fuse_level(const heal_act_t* feat, const float* occ, const double* theta,
                             const int* crop_windows, int n_agents, int H, int W, int C, int align_corners,
                             const long long* agent_feat_offsets_host, const long long* agent_occ_offsets_host,
                             int row0, int rows, const heal_act_t* out, void* stream);
 
-/* AttFusion.forward for one scene (opencood/models/fuse_modules/fusion_in_one.py:126-151) */
+/* AttFusion.forward for one scene (opencood/models/fuse_modules/fusion_in_one.py:126-151).  C in {128, 256, 384, 512},
+ * n_agents <= 8.  Alignment as heal_pyramid_fuse_level: strides, offsets and plane strides multiples of 4 elements, data
+ * 16-byte aligned (fp32) or 8-byte aligned (bf16 / split), else HEAL_ERR_UNSUPPORTED; split input with C <= 256, strides and
+ * offsets multiples of 8 and a 16-byte aligned data pointer takes the 8-channel kernel. */
 int heal_att_fuse(const heal_act_t* feat, const double* theta, int n_agents, int H, int W, int C,
                   const heal_act_t* out, void* stream);
 
 /* MaxFusion.forward for one scene (fusion_in_one.py:87-124): out(H,W,C) = max over j of warp(feat_j, theta[j]).
  * Pixels warped in from outside agent j's map are 0 and take part in the max.  feat (n,H,W,C), theta (n,2,3) fp64 device;
- * C, channel strides and offsets multiples of 4. */
+ * C, channel strides, offsets and plane strides multiples of 4; feat->data / out->data 16-byte aligned for fp32, 8-byte
+ * aligned for bf16 / split (else HEAL_ERR_UNSUPPORTED). */
 int heal_max_fuse(const heal_act_t* feat, const double* theta, int n_agents, int H, int W, int C,
                   const heal_act_t* out, void* stream);
 
 /* A batch of warp_affine_simple (bilinear, zeros padding, align_corners=False):
  * out image k = grid_sample(src image src_index_host[k], theta[k]) for k < n_out.
- * src_index_host: HOST array of n_out image indices into src (H,W,C maps); theta (n_out,2,3) fp64 device; out (n_out,H,W,C). */
+ * src_index_host: HOST array of n_out image indices into src (H,W,C maps); theta (n_out,2,3) fp64 device; out (n_out,H,W,C).
+ * Alignment of src and out as heal_max_fuse. */
 int heal_warp_affine(const heal_act_t* src, const int* src_index_host, const double* theta, int n_out,
                      int H, int W, int C, const heal_act_t* out, void* stream);
 
@@ -196,13 +205,14 @@ int heal_warp_affine(const heal_act_t* src, const int* src_index_host, const dou
  *   msg_j = mask_j * (q[r + j] + p_node[P image]),  mask_j = warp(ones, theta[r + j]) (recomputed from the taps)
  *   agg   = mean_j msg_j (agg_max = 0, divides by n) or max_j msg_j (agg_max = 1)
  * gru = 1: out image u (2C channels) = [x | agg]  (the ConvGRU input);  gru = 0: out image u (C channels) = x + agg.
- * q (pairs,H,W,C) = W[:, :C] (*) warped neighbours; p_node (.,H,W,C) = W[:, C:] (*) x + bias; theta (pairs,2,3) fp64 device. */
+ * q (pairs,H,W,C) = W[:, :C] (*) warped neighbours; p_node (.,H,W,C) = W[:, C:] (*) x + bias; theta (pairs,2,3) fp64 device.
+ * Alignment of q, p_node, x and out as heal_max_fuse. */
 int heal_v2v_aggregate(const heal_act_t* q, const heal_act_t* p_node, const heal_act_t* x, const double* theta,
                        const int* nodes_host, int n_nodes, int H, int W, int C, int agg_max, int gru,
                        const heal_act_t* out, void* stream);
 
 /* ConvGRU cell with a zero hidden state (sub_modules/convgru.py:47-68): out(npix,C) = sigmoid(zc[:, :C]) * tanh(zc[:, C:2C]),
- * zc = the stacked (update gate | candidate) GRU conv output (npix, 2C). */
+ * zc = the stacked (update gate | candidate) GRU conv output (npix, 2C).  Alignment of zc and out as heal_max_fuse. */
 int heal_gru_gate(const heal_act_t* zc, long long npix, int C, const heal_act_t* out, void* stream);
 
 /* CoBEVT window / grid attention core (swap_fusion_modules.py:87-128 with CoBEVT's agent mask, fusion_in_one.py:409-429).
