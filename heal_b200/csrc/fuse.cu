@@ -396,6 +396,127 @@ k_att_fuse_split8(AttP p) {
     }
 }
 
+// 8 channels of a pixel with 16 B stores per plane (fp32: two float4); the rounding of act_store4.
+__device__ __forceinline__ void act_store8(const ActV& a, size_t pix, int c, const float (&v)[8]) {
+    const size_t idx = pix * (size_t)a.cs + (size_t)(a.co + c);
+    if (a.fmt == 0) {
+        float4* f = reinterpret_cast<float4*>(reinterpret_cast<float*>(a.p) + idx);
+        f[0] = make_float4(v[0], v[1], v[2], v[3]);
+        f[1] = make_float4(v[4], v[5], v[6], v[7]);
+        return;
+    }
+    __nv_bfloat16* b = reinterpret_cast<__nv_bfloat16*>(a.p) + idx;
+    uint4 h, l;
+    __nv_bfloat162* h2 = reinterpret_cast<__nv_bfloat162*>(&h);
+    __nv_bfloat162* l2 = reinterpret_cast<__nv_bfloat162*>(&l);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) h2[q] = __floats2bfloat162_rn(v[2 * q], v[2 * q + 1]);
+    *reinterpret_cast<uint4*>(b) = h;
+    if (a.fmt == 2) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const float2 hf = __bfloat1622float2(h2[q]);
+            l2[q] = __floats2bfloat162_rn(v[2 * q] - hf.x, v[2 * q + 1] - hf.y);
+        }
+        *reinterpret_cast<uint4*>(b + a.plane) = l;
+    }
+}
+
+// C = 64 (the first level of the multi-scale models): 8 lanes per output pixel, 8 channels per lane, 4 pixels per warp and 16
+// per 128-thread block, so all 32 lanes load even though a pixel has only 64 channels.  FMT is the input format (0 f32,
+// 1 bf16, 2 split-bf16): each tap is 32 B per lane in fp32 (two float4), 16 B per plane otherwise.  Every agent's warped 8-channel
+// slice is sampled once (FMA over the taps in nw, ne, sw, se order, as in k_att_fuse_split8) and kept in registers for both the
+// ego-row scores and the weighted sum; the score is reduced over the pixel's 8 lanes with 3 xor shuffles.
+template <int NA, int FMT>
+__global__ void __launch_bounds__(128)
+k_att_fuse_g8(AttP p) {
+    const int HW = p.H * p.W;
+    if (blockIdx.x * 16 + (threadIdx.x >> 5) * 4 >= HW) return;      // whole warp past the map (the shuffles need all 32 lanes)
+    const int pix_raw = blockIdx.x * 16 + (threadIdx.x >> 3);
+    const bool valid = pix_raw < HW;
+    const int pix = valid ? pix_raw : HW - 1;                        // a partial warp's tail lanes recompute the last pixel
+    const int c0 = 8 * (threadIdx.x & 7);
+    constexpr int R = FMT == 1 ? 1 : 2;                              // uint4 per tap: fp32 8 floats, split hi + lo, bf16 hi
+    const size_t lo_off = FMT == 2 ? p.feat.plane : 0;
+    float xs[NA][8];
+    float sc[NA];
+    float mx = -INFINITY;
+#pragma unroll
+    for (int j = 0; j < NA; ++j) {
+        if (j < p.n) {
+            const Tap t = make_tap(p.theta + 6 * j, pix / p.W, pix % p.W, p.H, p.W, p.align);
+            uint4 v[4][R];
+            float w[4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+#pragma unroll
+                for (int r = 0; r < R; ++r) v[k][r] = make_uint4(0u, 0u, 0u, 0u);
+                w[k] = t.w[k];
+                if (t.off[k] >= 0) {
+                    const size_t e = ((size_t)j * HW + t.off[k]) * (size_t)p.feat.cs + (size_t)(p.feat.co + c0);
+                    if (FMT == 0) {
+                        const uint4* f = reinterpret_cast<const uint4*>(reinterpret_cast<const float*>(p.feat.p) + e);
+                        v[k][0] = __ldg(f);
+                        v[k][R - 1] = __ldg(f + 1);
+                    } else {
+                        const __nv_bfloat16* h = reinterpret_cast<const __nv_bfloat16*>(p.feat.p) + e;
+                        v[k][0] = __ldg(reinterpret_cast<const uint4*>(h));
+                        if (FMT == 2) v[k][R - 1] = __ldg(reinterpret_cast<const uint4*>(h + lo_off));
+                    }
+                } else {
+                    w[k] = 0.f;
+                }
+            }
+#pragma unroll
+            for (int e = 0; e < 8; ++e) xs[j][e] = 0.f;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                float x[8];
+                const uint32_t* a32 = reinterpret_cast<const uint32_t*>(&v[k][0]);
+                const uint32_t* b32 = reinterpret_cast<const uint32_t*>(&v[k][R - 1]);
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    if (FMT == 0) {
+                        x[q] = __uint_as_float(a32[q]);
+                        x[4 + q] = __uint_as_float(b32[q]);
+                    } else if (FMT == 1) {
+                        x[2 * q] = __uint_as_float(a32[q] << 16);
+                        x[2 * q + 1] = __uint_as_float(a32[q] & 0xffff0000u);
+                    } else {
+                        x[2 * q] = __uint_as_float(a32[q] << 16) + __uint_as_float(b32[q] << 16);
+                        x[2 * q + 1] = __uint_as_float(a32[q] & 0xffff0000u) + __uint_as_float(b32[q] & 0xffff0000u);
+                    }
+                }
+#pragma unroll
+                for (int e = 0; e < 8; ++e) xs[j][e] = fmaf(x[e], w[k], xs[j][e]);
+            }
+            float d = 0.f;
+#pragma unroll
+            for (int e = 0; e < 8; ++e) d += xs[0][e] * xs[j][e];
+#pragma unroll
+            for (int o = 4; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
+            d *= p.inv_sqrt_dim;
+            sc[j] = d;
+            mx = fmaxf(mx, d);
+        }
+    }
+    float den = 0.f;
+#pragma unroll
+    for (int j = 0; j < NA; ++j) if (j < p.n) { sc[j] = expf(sc[j] - mx); den += sc[j]; }
+    float acc[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc[e] = 0.f;
+#pragma unroll
+    for (int j = 0; j < NA; ++j) {
+        if (j < p.n) {
+            const float a = sc[j] / den;
+#pragma unroll
+            for (int e = 0; e < 8; ++e) acc[e] = fmaf(a, xs[j][e], acc[e]);
+        }
+    }
+    if (valid) act_store8(p.out, (size_t)pix, c0, acc);
+}
+
 // ---- MaxFusion / V2VNetFusion (fusion_in_one.py:87-124, :203-318) ---------------------------------------------------------
 // One thread per (image, pixel, 4-channel chunk); blockIdx.y is the image inside the launch.  Every thread recomputes its taps
 // with make_tap (a few fp64 FMAs), so the arithmetic per tap is the one the attention / pyramid kernels use.
@@ -528,6 +649,19 @@ static inline bool aligned8_split(const heal_act_t* a) {
     return a->fmt == 2 && ((uintptr_t)a->data & 15) == 0 && (a->cstride & 7) == 0 && (a->coffset & 7) == 0 &&
            (a->plane_stride & 7) == 0;
 }
+// k_att_fuse_g8 loads and stores 16 B per plane and 8-channel group: a 16 B-aligned base, channel groups of 8 in bf16 / split
+// (fp32 reads two float4, so groups of 4 do, which is aligned4).
+static inline bool aligned16(const heal_act_t* a) {
+    if (a->fmt == 0) return aligned4(a);
+    return (a->fmt == 1 || a->fmt == 2) && ((uintptr_t)a->data & 15) == 0 && (a->cstride & 7) == 0 && (a->coffset & 7) == 0 &&
+           (a->fmt == 1 || (a->plane_stride & 7) == 0);
+}
+
+template <int FMT>
+static void launch_att_g8(const AttP& p, int grid, cudaStream_t st) {
+    if (p.n <= 5) k_att_fuse_g8<5, FMT><<<grid, 128, 0, st>>>(p);         // register file sized for the scene
+    else k_att_fuse_g8<MAX_AGENTS, FMT><<<grid, 128, 0, st>>>(p);
+}
 
 extern "C" int heal_pyramid_fuse_level(const heal_act_t* feat, const float* occ, const double* theta,
                                        const int* crop_windows, int n_agents, int H, int W, int C, int align_corners,
@@ -570,11 +704,22 @@ extern "C" int heal_att_fuse(const heal_act_t* feat, const double* theta, int n_
                              const heal_act_t* out, void* stream_) {
     if (!feat || !feat->data || !theta || !out || !out->data) return HEAL_ERR_ARG;
     if (n_agents < 1 || n_agents > MAX_AGENTS) return HEAL_ERR_UNSUPPORTED;
-    if ((C % 128) || C > 512 || !aligned4(feat) || !aligned4(out)) return HEAL_ERR_UNSUPPORTED;
+    if (C == 64) {
+        if (!aligned16(feat) || !aligned16(out)) return HEAL_ERR_UNSUPPORTED;
+    } else if ((C % 128) || C > 512 || !aligned4(feat) || !aligned4(out)) {
+        return HEAL_ERR_UNSUPPORTED;
+    }
     AttP p;
     p.feat = to_view(feat); p.theta = theta; p.out = to_view(out); p.n = n_agents; p.H = H; p.W = W; p.C = C; p.align = 0;
     p.inv_sqrt_dim = 1.0f / sqrtf((float)C);
     cudaStream_t st = (cudaStream_t)stream_;
+    if (C == 64) {
+        const int grid = (H * W + 15) / 16;
+        if (feat->fmt == 0) launch_att_g8<0>(p, grid, st);
+        else if (feat->fmt == 1) launch_att_g8<1>(p, grid, st);
+        else launch_att_g8<2>(p, grid, st);
+        return heal_check_launch();
+    }
     if (aligned8_split(feat) && C <= 256) {
         if (n_agents <= 5) k_att_fuse_split8<5><<<(H * W + 3) / 4, 128, 0, st>>>(p);       // register file sized for the scene
         else k_att_fuse_split8<MAX_AGENTS><<<(H * W + 3) / 4, 128, 0, st>>>(p);

@@ -7,6 +7,7 @@ import sys
 _MAP = {
     "opencood.models.heter_pyramid_collab": "heal_b200.models.heter_pyramid_collab",
     "opencood.models.heter_model_baseline": "heal_b200.models.heter_model_baseline",
+    "opencood.models.heter_model_baseline_ms": "heal_b200.models.heter_model_baseline_ms",
     "opencood.models.point_pillar": "heal_b200.models.point_pillar",
     "opencood.models.heter_encoders": "heal_b200.models.heter_encoders",
     "opencood.models.fuse_modules.pyramid_fuse": "heal_b200.models.fuse_modules.pyramid_fuse",

@@ -182,7 +182,10 @@ int heal_pyramid_fuse_level(const heal_act_t* feat, const float* occ, const doub
 /* AttFusion.forward for one scene (opencood/models/fuse_modules/fusion_in_one.py:126-151).  C in {128, 256, 384, 512},
  * n_agents <= 8.  Alignment as heal_pyramid_fuse_level: strides, offsets and plane strides multiples of 4 elements, data
  * 16-byte aligned (fp32) or 8-byte aligned (bf16 / split), else HEAL_ERR_UNSUPPORTED; split input with C <= 256, strides and
- * offsets multiples of 8 and a 16-byte aligned data pointer takes the 8-channel kernel. */
+ * offsets multiples of 8 and a 16-byte aligned data pointer takes the 8-channel kernel.  C = 64 (the first level of
+ * HeterModelBaselineMs) takes its own kernel, for every input format, with 16-byte loads and stores: input and output data
+ * 16-byte aligned and, for bf16 / split, strides, offsets and plane strides multiples of 8 (fp32: of 4), else
+ * HEAL_ERR_UNSUPPORTED. */
 int heal_att_fuse(const heal_act_t* feat, const double* theta, int n_agents, int H, int W, int C,
                   const heal_act_t* out, void* stream);
 
