@@ -13,6 +13,7 @@ channels-last (`x.permute(0,2,3,1)` contiguous), which keeps the reference's sha
 from __future__ import annotations
 
 import ctypes
+import functools
 from typing import Optional, Sequence
 
 import numpy as np
@@ -29,15 +30,55 @@ def _p(t: Optional[torch.Tensor]):
 
 
 def _stream():
-    """Current stream of the CURRENT device.  Every public wrapper runs under `_on(tensor)` (see below), which makes the
+    """Current stream of the CURRENT device.  Every public wrapper that launches is decorated with `_guard`, which makes the
     tensors' device current first, so the launch, the stream and the per-device kernel attributes all agree."""
     return _vp(torch.cuda.current_stream().cuda_stream)
 
 
-def _on(t):
-    """Context manager: make `t`'s device current for the duration of a C-ABI call (the library launches on the current device)."""
-    dev = t.device if hasattr(t, "device") else t
-    return torch.cuda.device(dev)
+def _call(symbol: str, *args):
+    """Launch `symbol` of libheal_b200.so on the current stream (appended as the last argument); raise on an error code.
+    Pass `Act.view()` results as they are: ctypes passes a HealAct by reference where the argtype is a pointer to it."""
+    check(getattr(lib, symbol)(*args, _stream()), symbol)
+
+
+# ------------------------------------------------------------------------------------------------
+# device guard: the library launches on the CURRENT device and on the stream passed in; every public wrapper that launches
+# therefore runs with its tensors' device made current (a model on cuda:1 while cuda:0 is current, or one process driving
+# two GPUs).
+# ------------------------------------------------------------------------------------------------
+def _device_of(x):
+    if isinstance(x, torch.Tensor):
+        return x.device if x.is_cuda else None
+    if isinstance(x, (Act, SparseCanvas)):
+        return x.device
+    if isinstance(x, SparseTensor):
+        return x.coords.device
+    return None
+
+
+def _first_device_arg(*args, **kwargs):
+    """The first argument, positional then keyword, that carries a CUDA device."""
+    for a in (*args, *kwargs.values()):
+        if _device_of(a) is not None:
+            return a
+    return None
+
+
+def _guard(fn=None, *, device_arg=_first_device_arg):
+    """Decorator: run `fn` with the device of `device_arg(*args, **kwargs)` current (no device context when it already
+    is).  The wrapper keeps `device_arg` as an attribute, which marks it as guarded."""
+    if fn is None:
+        return functools.partial(_guard, device_arg=device_arg)
+
+    @functools.wraps(fn)
+    def wrapped(*args, **kwargs):
+        dev = _device_of(device_arg(*args, **kwargs))
+        if dev is None or dev.index is None or dev.index == torch.cuda.current_device():
+            return fn(*args, **kwargs)
+        with torch.cuda.device(dev):
+            return fn(*args, **kwargs)
+    wrapped.device_arg = device_arg
+    return wrapped
 
 
 def _need_cuda(*ts):
@@ -145,20 +186,43 @@ class Act:
         return Act(self.t[:, a:b] if self.fmt == "f32" else self.t[:, :, a:b], self.fmt)
 
 
-def act_empty(N, H, W, C, fmt: str, device) -> Act:
+def _act_new(new, N, H, W, C, fmt: str, device) -> Act:
     if fmt == "f32":
-        return Act(torch.empty((N, H, W, C), dtype=torch.float32, device=device), fmt)
-    return Act(torch.empty((2 if fmt == "split" else 1, N, H, W, C), dtype=torch.bfloat16, device=device), fmt)
+        return Act(new((N, H, W, C), dtype=torch.float32, device=device), fmt)
+    return Act(new((2 if fmt == "split" else 1, N, H, W, C), dtype=torch.bfloat16, device=device), fmt)
 
 
+def act_empty(N, H, W, C, fmt: str, device) -> Act:
+    return _act_new(torch.empty, N, H, W, C, fmt, device)
+
+
+def act_zeros(N, H, W, C, fmt: str, device) -> Act:
+    """Zero-filled Act (all-zero bits are 0.0 in every storage format): a canvas the kernel writes at hit cells only."""
+    return _act_new(torch.zeros, N, H, W, C, fmt, device)
+
+
+def _out_act(out: Optional[Act], N, H, W, C, fmt: str, device) -> Act:
+    """A wrapper's whole-tensor output: `out` when given (it must be (N,H,W,C)), else a new Act in `fmt`."""
+    if out is None:
+        return act_empty(N, H, W, C, fmt, device)
+    assert (out.N, out.H, out.W, out.C) == (N, H, W, C)
+    return out
+
+
+def _theta64(theta: torch.Tensor, n: int) -> torch.Tensor:
+    """(n,2,3) affine poses as the contiguous fp64 array the fusion kernels read."""
+    th = theta.to(torch.float64).contiguous()
+    assert th.shape == (n, 2, 3)
+    return th
+
+
+@_guard
 def convert(a: Act, fmt: str) -> Act:
     if a.fmt == fmt:
         return a
     out = act_empty(a.N, a.H, a.W, a.C, fmt, a.device)
-    sv, dv = a.view(), out.view()
     with _Prof("act_convert", 0, a.N * a.H * a.W * float(a.C) * (BPE[a.fmt] + BPE[fmt])):
-        rc = lib.heal_act_convert(ctypes.byref(sv), ctypes.byref(dv), a.N * a.H * a.W, a.C, _stream())
-    check(rc, "heal_act_convert")
+        _call("heal_act_convert", a.view(), out.view(), a.N * a.H * a.W, a.C)
     return out
 
 
@@ -207,6 +271,7 @@ def grid_size_of(lidar_range, voxel_size):
     return np.round(g).astype(np.int64)
 
 
+@_guard
 def voxelize(points: torch.Tensor, agent_offsets: torch.Tensor, lidar_range, voxel_size,
              max_points_per_voxel: int, max_voxels: int, capacity: Optional[int] = None):
     """GPU SpVoxelPreprocessor.preprocess + collate for all agents of a scene.
@@ -230,14 +295,13 @@ def voxelize(points: torch.Tensor, agent_offsets: torch.Tensor, lidar_range, vox
     ws_bytes = lib.heal_voxelize_workspace(P, cap, A)
     ws = _workspace(dev, ws_bytes)
     with _Prof("voxelize", 0, lambda: 16.0 * P + float(nvox[0].item()) * (16 * T + 20)):
-        rc = lib.heal_voxelize(_p(points), _p(agent_offsets), A, P,
-                               _host_f32(lidar_range[0:3]), _host_f32(voxel_size), _host_i32(grid),
-                               T, int(max_voxels), cap, _p(voxels), _p(coords), _p(npts), _p(nvox),
-                               _p(ws), ws.numel(), _stream())
-    check(rc, "heal_voxelize")
+        _call("heal_voxelize", _p(points), _p(agent_offsets), A, P,
+              _host_f32(lidar_range[0:3]), _host_f32(voxel_size), _host_i32(grid),
+              T, int(max_voxels), cap, _p(voxels), _p(coords), _p(npts), _p(nvox), _p(ws), ws.numel())
     return voxels, coords, npts, nvox
 
 
+@_guard
 def mask_points(points: torch.Tensor, agent_offsets: torch.Tensor, lidar_range, remove_ego: bool = True,
                 perm: Optional[torch.Tensor] = None):
     """shuffle_points (host-drawn `perm`, optional) -> mask_ego_points -> mask_points_by_range on the GPU (pcd_utils.py:41-95), a
@@ -251,9 +315,8 @@ def mask_points(points: torch.Tensor, agent_offsets: torch.Tensor, lidar_range, 
     ws = _workspace(points.device, lib.heal_mask_points_workspace(P))
     pm = perm.to(torch.int32).contiguous() if perm is not None else None
     with _Prof("mask_points", 0, 32.0 * P):
-        rc = lib.heal_mask_points(_p(points), _p(pm), _p(agent_offsets), A, P, _host_f32(lidar_range), 1 if remove_ego else 0,
-                                  _p(out), _p(offs_out), _p(ws), ws.numel(), _stream())
-    check(rc, "heal_mask_points")
+        _call("heal_mask_points", _p(points), _p(pm), _p(agent_offsets), A, P, _host_f32(lidar_range), 1 if remove_ego else 0,
+              _p(out), _p(offs_out), _p(ws), ws.numel())
     return out, offs_out
 
 
@@ -271,6 +334,7 @@ def trim_voxels(voxels, coords, npts, nvox):
     return {"voxel_features": voxels[:m], "voxel_coords": coords[:m], "voxel_num_points": npts[:m]}
 
 
+@_guard
 def mean_vfe(voxels: torch.Tensor, num_points: torch.Tensor) -> torch.Tensor:
     _need_cuda(voxels, num_points)
     M, T, C = voxels.shape
@@ -278,8 +342,7 @@ def mean_vfe(voxels: torch.Tensor, num_points: torch.Tensor) -> torch.Tensor:
     npts = num_points.to(torch.int32).contiguous()
     out = torch.empty((M, 4), dtype=torch.float32, device=voxels.device)
     with _Prof("mean_vfe", 0, M * (T * 16.0 + 4 + 16)):
-        rc = lib.heal_mean_vfe(_p(voxels), _p(npts), M, T, _p(out), _stream())
-    check(rc, "heal_mean_vfe")
+        _call("heal_mean_vfe", _p(voxels), _p(npts), M, T, _p(out))
     return out
 
 
@@ -295,6 +358,7 @@ def fold_linear_bn(weight: torch.Tensor, bn_w, bn_b, bn_mean, bn_var, eps: float
     return wf.float(), shift.float()
 
 
+@_guard
 def pillar_vfe_scatter(voxel_features, voxel_num_points, voxel_coords, w_folded, b_folded,
                        voxel_size, lidar_range, nx: int, ny: int, batch_size: int,
                        want_pillar_features: bool = False, want_canvas: bool = True,
@@ -322,22 +386,14 @@ def pillar_vfe_scatter(voxel_features, voxel_num_points, voxel_coords, w_folded,
         return b
     with _Prof("pillar_vfe_scatter" + ("(+canvas memset)" if want_canvas else ""), lambda: 2.0 * T * w_folded.shape[0] * cout *
                (float(num_voxels_dev[0].item()) if num_voxels_dev is not None else float(M)), _bytes):
-        canvas, cview = None, None
-        if want_canvas:
-            if canvas_fmt == "f32":
-                canvas = Act(torch.zeros((batch_size, ny, nx, cout), dtype=torch.float32, device=dev), "f32")
-            else:
-                canvas = Act(torch.zeros((2 if canvas_fmt == "split" else 1, batch_size, ny, nx, cout),
-                                         dtype=torch.bfloat16, device=dev), canvas_fmt)
-            cv = canvas.view()
-            cview = ctypes.byref(cv)
-        rc = lib.heal_pillar_vfe_scatter(_p(vf), _p(npts), _p(coords), _p(num_voxels_dev), M, T,
-                                         _p(w_folded), _p(b_folded), w_folded.shape[0], cout,
-                                         _host_f32(vs), _host_f32(off), int(nx), int(ny), _p(pf), _p(split_rows_out), cview, _stream())
-    check(rc, "heal_pillar_vfe_scatter")
+        canvas = act_zeros(batch_size, ny, nx, cout, canvas_fmt, dev) if want_canvas else None
+        _call("heal_pillar_vfe_scatter", _p(vf), _p(npts), _p(coords), _p(num_voxels_dev), M, T,
+              _p(w_folded), _p(b_folded), w_folded.shape[0], cout, _host_f32(vs), _host_f32(off), int(nx), int(ny),
+              _p(pf), _p(split_rows_out), canvas.view() if canvas is not None else None)
     return pf, canvas
 
 
+@_guard
 def pillar_scatter(pillar_features: torch.Tensor, voxel_coords: torch.Tensor, nx: int, ny: int, batch_size: int,
                    fmt: str = "f32", num_voxels_dev: Optional[torch.Tensor] = None) -> Act:
     """Stand-alone PointPillarScatter: (M,C) f32 rows -> Act (B,ny,nx,C) (zero elsewhere)."""
@@ -345,13 +401,8 @@ def pillar_scatter(pillar_features: torch.Tensor, voxel_coords: torch.Tensor, nx
     M, C = pillar_features.shape
     coords = voxel_coords.to(torch.int32).contiguous()
     with _Prof("pillar_scatter(+canvas memset)", 0, M * (C * 4.0 + 16) + batch_size * float(ny) * nx * C * BPE[fmt]):
-        if fmt == "f32":
-            canvas = Act(torch.zeros((batch_size, ny, nx, C), dtype=torch.float32, device=coords.device), "f32")
-        else:
-            canvas = Act(torch.zeros((2 if fmt == "split" else 1, batch_size, ny, nx, C), dtype=torch.bfloat16, device=coords.device), fmt)
-        cv = canvas.view()
-        rc = lib.heal_pillar_scatter(_p(pillar_features), _p(coords), _p(num_voxels_dev), M, C, int(nx), int(ny), ctypes.byref(cv), _stream())
-    check(rc, "heal_pillar_scatter")
+        canvas = act_zeros(batch_size, ny, nx, C, fmt, coords.device)
+        _call("heal_pillar_scatter", _p(pillar_features), _p(coords), _p(num_voxels_dev), M, C, int(nx), int(ny), canvas.view())
     return canvas
 
 
@@ -512,6 +563,7 @@ def pack_conv_tc(conv, bn, relu: bool, planes: int = 2, extra_pad: int = 0) -> P
 # ------------------------------------------------------------------------------------------------
 # conv2d launchers
 # ------------------------------------------------------------------------------------------------
+@_guard
 def conv2d_simt(x: Act, pc: PackedConv, residual: Optional[Act] = None, out: Optional[Act] = None,
                 out_fmt: str = "f32", out_coffset: int = 0, in_coffset: int = 0, cin: Optional[int] = None) -> Act:
     """fp32 CUDA-core conv; any storage format in/out."""
@@ -529,7 +581,6 @@ def conv2d_simt(x: Act, pc: PackedConv, residual: Optional[Act] = None, out: Opt
         assert (residual.N, residual.H, residual.W) == (out.N, out.H, out.W)
     xv, ov = x.view(in_coffset), out.view(out_coffset)
     rv = residual.view() if residual is not None else None
-    st = _stream()
     fam = ("conv_grouped3x3_simt" if pc.groups > 1 else f"conv_dense{pc.kh}x{pc.kw}_simt")
     flops = 2.0 * N * Ho * Wo * pc.cout * (cin // pc.groups) * pc.kh * pc.kw * up * up
     nbytes = N * H * W * cin * BPE[x.fmt] + N * out.H * out.W * pc.cout * BPE[out.fmt] + pc.weight.numel() * 4.0 \
@@ -538,14 +589,12 @@ def conv2d_simt(x: Act, pc: PackedConv, residual: Optional[Act] = None, out: Opt
         for i in range(up):
             for j in range(up):
                 wptr = pc.weight if up == 1 else pc.weight[i, j]
-                rc = lib.heal_conv2d_simt(ctypes.byref(xv), N, H, W, cin, _p(wptr), pc.w_cstride, _p(pc.bias),
-                                          pc.kh, pc.kw, pc.stride, pc.pad, pc.groups,
-                                          ctypes.byref(rv) if rv is not None else None, ctypes.byref(ov),
-                                          Ho, Wo, pc.cout, up, i, j, int(pc.relu), st)
-                check(rc, "heal_conv2d_simt")
+                _call("heal_conv2d_simt", xv, N, H, W, cin, _p(wptr), pc.w_cstride, _p(pc.bias), pc.kh, pc.kw, pc.stride,
+                      pc.pad, pc.groups, rv, ov, Ho, Wo, pc.cout, up, i, j, int(pc.relu))
     return out
 
 
+@_guard
 def conv2d_tc(x: Act, pc: PackedConvTC, residual: Optional[Act] = None, out: Optional[Act] = None,
               out_coffset: int = 0, in_coffset: int = 0, want_split: bool = True,
               out_f32: Optional[Act] = None, want_f32: bool = False, out32_coffset: int = 0):
@@ -575,19 +624,19 @@ def conv2d_tc(x: Act, pc: PackedConvTC, residual: Optional[Act] = None, out: Opt
         + (N * Ho * Wo * up * up * pc.cout * 4.0 if out_f32 is not None else 0) \
         + (N * Ho * Wo * up * up * pc.cout * BPE[residual.fmt] if residual is not None else 0)
     with _Prof(fam, flops, nbytes):
-        rc = lib.heal_conv2d_tc(_p(x.t), x.plane_stride, N, H, W, pc.cin, x.cstride, in_coffset,
-                                _p(pc.w), _p(pc.w_diag), pc.w.shape[1], pc.coutp, _p(pc.bias), pc.kh, pc.kw, pc.stride, pc.pad,
-                                1 if pc.blockdiag else 0, x.planes, pc.planes,
-                                _p(res_split), res_plane, _p(res_f32), res_cs, 0,
-                                _p(out.t) if out is not None else _vp(0), out.plane_stride if out is not None else 0,
-                                out.cstride if out is not None else 0, out_coffset,
-                                _p(out_f32.t) if out_f32 is not None else _vp(0),
-                                out_f32.cstride if out_f32 is not None else 0, out32_coffset,
-                                Ho, Wo, pc.cout, up, int(pc.relu), _stream())
-    check(rc, "heal_conv2d_tc")
+        _call("heal_conv2d_tc", _p(x.t), x.plane_stride, N, H, W, pc.cin, x.cstride, in_coffset,
+              _p(pc.w), _p(pc.w_diag), pc.w.shape[1], pc.coutp, _p(pc.bias), pc.kh, pc.kw, pc.stride, pc.pad,
+              1 if pc.blockdiag else 0, x.planes, pc.planes,
+              _p(res_split), res_plane, _p(res_f32), res_cs, 0,
+              _p(out.t) if out is not None else _vp(0), out.plane_stride if out is not None else 0,
+              out.cstride if out is not None else 0, out_coffset,
+              _p(out_f32.t) if out_f32 is not None else _vp(0),
+              out_f32.cstride if out_f32 is not None else 0, out32_coffset,
+              Ho, Wo, pc.cout, up, int(pc.relu))
     return out, out_f32
 
 
+@_guard
 def bottleneck_tc(x: Act, pc1: PackedConvTC, pc2: PackedConvTC, pc3: PackedConvTC, out: Optional[Act] = None,
                   out_coffset: int = 0) -> Act:
     """ResNeXt bottleneck ReLU(conv3(conv2(conv1(x))) + x) in one kernel (64 -> 128 -> 64 channels, grouped 3x3, stride 1):
@@ -605,16 +654,16 @@ def bottleneck_tc(x: Act, pc1: PackedConvTC, pc2: PackedConvTC, pc3: PackedConvT
     epb = 2.0 * x.planes
     nbytes = 2.0 * N * H * W * C * epb + 2.0 * (pc1.w.numel() + pc2.w_diag.numel() + pc3.w.numel())
     with _Prof("conv_tc_bottleneck", flops, nbytes):
-        rc = lib.heal_bottleneck_tc(_p(x.t), x.plane_stride, N, H, W, C, x.cstride,
-                                    _p(pc1.w), _p(pc1.bias), _p(pc2.w_diag), _p(pc2.bias), _p(pc3.w), _p(pc3.bias),
-                                    x.planes, pc1.planes, _p(out.t), out.plane_stride, out.cstride, out_coffset, _stream())
-    check(rc, "heal_bottleneck_tc")
+        _call("heal_bottleneck_tc", _p(x.t), x.plane_stride, N, H, W, C, x.cstride,
+              _p(pc1.w), _p(pc1.bias), _p(pc2.w_diag), _p(pc2.bias), _p(pc3.w), _p(pc3.bias),
+              x.planes, pc1.planes, _p(out.t), out.plane_stride, out.cstride, out_coffset)
     return out
 
 
 # ------------------------------------------------------------------------------------------------
 # ConvNeXt aligner front half, ResNet-stem max pooling
 # ------------------------------------------------------------------------------------------------
+@_guard
 def dwconv_layernorm(x: Act, dw_weight: torch.Tensor, dw_bias, ksize: int, ln_weight, ln_bias, eps: float,
                      out_fmt: Optional[str] = None) -> Act:
     """depthwise ksize x ksize conv (+bias) + LayerNorm over channels.  dw_weight (ksize*ksize, C) fp32 tap-major."""
@@ -622,15 +671,14 @@ def dwconv_layernorm(x: Act, dw_weight: torch.Tensor, dw_bias, ksize: int, ln_we
     N, H, W, C = x.N, x.H, x.W, x.C
     assert dw_weight.shape == (ksize * ksize, C) and dw_weight.is_contiguous()
     out = act_empty(N, H, W, C, out_fmt or x.fmt, x.device)
-    xv, ov = x.view(), out.view()
     lw, lb = ln_weight.float().contiguous(), ln_bias.float().contiguous()
     with _Prof("dwconv_layernorm", 2.0 * N * H * W * C * ksize * ksize, N * H * W * float(C) * (BPE[x.fmt] + BPE[out.fmt])):
-        rc = lib.heal_dwconv_layernorm(ctypes.byref(xv), N, H, W, C, _p(dw_weight), _p(dw_bias), int(ksize), _p(lw), _p(lb),
-                                       float(eps), ctypes.byref(ov), _stream())
-    check(rc, "heal_dwconv_layernorm")
+        _call("heal_dwconv_layernorm", x.view(), N, H, W, C, _p(dw_weight), _p(dw_bias), int(ksize), _p(lw), _p(lb),
+              float(eps), out.view())
     return out
 
 
+@_guard
 def maxpool3x3s2(x: Act, out_fmt: Optional[str] = None, depth_to_space_in: bool = False) -> Act:
     """3x3 / stride 2 / pad 1 max pooling (torchvision ResNet stem).  depth_to_space_in: x is (N,H/2,W/2,4C) phase-major
     (channel block (y&1)*2+(x&1)) and stands for the logical (N,H,W,C) map."""
@@ -639,16 +687,15 @@ def maxpool3x3s2(x: Act, out_fmt: Optional[str] = None, depth_to_space_in: bool 
         H, W, C = 2 * H, 2 * W, C // 4
     Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
     out = act_empty(N, Ho, Wo, C, out_fmt or x.fmt, x.device)
-    xv, ov = x.view(), out.view()
     with _Prof("maxpool3x3s2", 0, N * float(C) * (H * W * BPE[x.fmt] + Ho * Wo * BPE[out.fmt])):
-        rc = lib.heal_maxpool3x3s2(ctypes.byref(xv), N, H, W, C, 1 if depth_to_space_in else 0, ctypes.byref(ov), _stream())
-    check(rc, "heal_maxpool3x3s2")
+        _call("heal_maxpool3x3s2", x.view(), N, H, W, C, 1 if depth_to_space_in else 0, out.view())
     return out
 
 
 # ------------------------------------------------------------------------------------------------
 # fusion
 # ------------------------------------------------------------------------------------------------
+@_guard
 def pyramid_fuse_level(feat: Act, occ: torch.Tensor, theta: torch.Tensor, align_corners: bool,
                        crop_windows: Optional[torch.Tensor] = None, out: Optional[Act] = None,
                        out_fmt: Optional[str] = None, out_coffset: int = 0,
@@ -662,73 +709,62 @@ def pyramid_fuse_level(feat: Act, occ: torch.Tensor, theta: torch.Tensor, align_
     assert occ.dtype == torch.float32
     if agent_offsets is None:
         assert occ.is_contiguous() and occ.numel() == n * H * W
-    th = theta.to(torch.float64).contiguous()
-    assert th.shape == (n, 2, 3)
+    th = _theta64(theta, n)
     row0, nrows = rows if rows is not None else (0, H)
     if out is None:
         out = act_empty(1, nrows, W, C, out_fmt or feat.fmt, feat.device)
     assert out.H == nrows and out.W == W
     cw = crop_windows.to(torch.int32).contiguous() if crop_windows is not None else None
-    fv, ov = feat.view(), out.view(out_coffset)
     fo = oo = None
     if agent_offsets is not None:
         fo = (ctypes.c_longlong * n)(*[int(v) for v in agent_offsets[0]])
         oo = (ctypes.c_longlong * n)(*[int(v) for v in agent_offsets[1]])
     with _Prof("pyramid_fuse_level", 0, (n * (C * BPE[feat.fmt] + 4.0) + C * BPE[out.fmt]) * float(nrows) * W):
-        rc = lib.heal_pyramid_fuse_level(ctypes.byref(fv), _p(occ), _p(th), _p(cw), n, H, W, C,
-                                         1 if align_corners else 0, fo, oo, int(row0), int(nrows), ctypes.byref(ov), _stream())
-    check(rc, "heal_pyramid_fuse_level")
+        _call("heal_pyramid_fuse_level", feat.view(), _p(occ), _p(th), _p(cw), n, H, W, C,
+              1 if align_corners else 0, fo, oo, int(row0), int(nrows), out.view(out_coffset))
     return out
 
 
+@_guard
 def att_fuse(feat: Act, theta: torch.Tensor, out: Optional[Act] = None, out_fmt: Optional[str] = None) -> Act:
     """feat: Act (n,H,W,C), theta (n,2,3) f64 -> Act (1,H,W,C)."""
     _need_cuda(theta)
     n, H, W, C = feat.N, feat.H, feat.W, feat.C
-    th = theta.to(torch.float64).contiguous()
-    if out is None:
-        out = act_empty(1, H, W, C, out_fmt or feat.fmt, feat.device)
-    fv, ov = feat.view(), out.view()
+    th = _theta64(theta, n)
+    out = _out_act(out, 1, H, W, C, out_fmt or feat.fmt, feat.device)
     with _Prof("att_fuse", 4.0 * n * C * H * W, (n * BPE[feat.fmt] + BPE[out.fmt]) * float(C) * H * W):
-        rc = lib.heal_att_fuse(ctypes.byref(fv), _p(th), n, H, W, C, ctypes.byref(ov), _stream())
-    check(rc, "heal_att_fuse")
+        _call("heal_att_fuse", feat.view(), _p(th), n, H, W, C, out.view())
     return out
 
 
+@_guard
 def max_fuse(feat: Act, theta: torch.Tensor, out: Optional[Act] = None, out_fmt: Optional[str] = None) -> Act:
     """MaxFusion of one scene: feat Act (n,H,W,C), theta (n,2,3) f64 -> Act (1,H,W,C) = max_j warp(feat_j, theta_j)."""
     _need_cuda(theta)
     n, H, W, C = feat.N, feat.H, feat.W, feat.C
-    th = theta.to(torch.float64).contiguous()
-    assert th.shape == (n, 2, 3)
-    if out is None:
-        out = act_empty(1, H, W, C, out_fmt or feat.fmt, feat.device)
-    assert (out.H, out.W, out.C) == (H, W, C)
-    fv, ov = feat.view(), out.view()
+    th = _theta64(theta, n)
+    out = _out_act(out, 1, H, W, C, out_fmt or feat.fmt, feat.device)
     with _Prof("max_fuse", 4.0 * n * C * H * W, (n * BPE[feat.fmt] + BPE[out.fmt]) * float(C) * H * W):
-        rc = lib.heal_max_fuse(ctypes.byref(fv), _p(th), n, H, W, C, ctypes.byref(ov), _stream())
-    check(rc, "heal_max_fuse")
+        _call("heal_max_fuse", feat.view(), _p(th), n, H, W, C, out.view())
     return out
 
 
+@_guard
 def warp_affine(src: Act, src_index: Sequence[int], theta: torch.Tensor, out: Optional[Act] = None,
                 out_fmt: Optional[str] = None) -> Act:
     """Batched warp_affine_simple (bilinear, zeros, align_corners=False): out image k = warp(src image src_index[k], theta[k]).
     src Act (n,H,W,C); theta (K,2,3) f64 on the device; `src_index` a host sequence of K image indices -> Act (K,H,W,C)."""
     _need_cuda(theta)
     K, H, W, C = len(src_index), src.H, src.W, src.C
-    th = theta.to(torch.float64).contiguous()
-    assert th.shape == (K, 2, 3) and all(0 <= int(s) < src.N for s in src_index)
-    if out is None:
-        out = act_empty(K, H, W, C, out_fmt or src.fmt, src.device)
-    assert (out.N, out.H, out.W, out.C) == (K, H, W, C)
-    sv, ov = src.view(), out.view()
+    th = _theta64(theta, K)
+    assert all(0 <= int(s) < src.N for s in src_index)
+    out = _out_act(out, K, H, W, C, out_fmt or src.fmt, src.device)
     with _Prof("warp_affine", 8.0 * K * C * H * W, K * (BPE[src.fmt] + BPE[out.fmt]) * float(C) * H * W):
-        rc = lib.heal_warp_affine(ctypes.byref(sv), _host_i32(src_index), _p(th), K, H, W, C, ctypes.byref(ov), _stream())
-    check(rc, "heal_warp_affine")
+        _call("heal_warp_affine", src.view(), _host_i32(src_index), _p(th), K, H, W, C, out.view())
     return out
 
 
+@_guard
 def v2v_aggregate(q: Act, p_node: Act, x: Act, theta: torch.Tensor, nodes: Sequence[Sequence[int]], agg_max: bool,
                   gru: bool, out: Optional[Act] = None, out_fmt: Optional[str] = None) -> Act:
     """V2VNet message aggregation.  nodes[u] = (x image, P image, first pair row r, neighbour count n) of updated node u;
@@ -736,41 +772,35 @@ def v2v_aggregate(q: Act, p_node: Act, x: Act, theta: torch.Tensor, nodes: Seque
     Act (U,H,W,C) = x + agg; agg = mean_j (agg_max False) or max_j of mask_j * (q[r + j] + p_node[P image])."""
     _need_cuda(theta)
     H, W, C, U = x.H, x.W, x.C, len(nodes)
-    th = theta.to(torch.float64).contiguous()
-    assert th.shape == (q.N, 2, 3) and (q.H, q.W, q.C) == (H, W, C) and (p_node.H, p_node.W, p_node.C) == (H, W, C)
+    th = _theta64(theta, q.N)
+    assert (q.H, q.W, q.C) == (H, W, C) and (p_node.H, p_node.W, p_node.C) == (H, W, C)
     flat = [int(v) for nd in nodes for v in nd]
     assert len(flat) == 4 * U
     cout = 2 * C if gru else C
-    if out is None:
-        out = act_empty(U, H, W, cout, out_fmt or x.fmt, x.device)
-    assert (out.N, out.H, out.W, out.C) == (U, H, W, cout)
+    out = _out_act(out, U, H, W, cout, out_fmt or x.fmt, x.device)
     pairs = float(sum(nd[3] for nd in nodes))
-    qv, pv, xv, ov = q.view(), p_node.view(), x.view(), out.view()
     with _Prof("v2v_aggregate", 3.0 * pairs * C * H * W,
                (pairs * BPE[q.fmt] + U * (BPE[p_node.fmt] + BPE[x.fmt]) + U * (cout // C) * BPE[out.fmt]) * float(C) * H * W):
-        rc = lib.heal_v2v_aggregate(ctypes.byref(qv), ctypes.byref(pv), ctypes.byref(xv), _p(th), _host_i32(flat), U, H, W, C,
-                                    1 if agg_max else 0, 1 if gru else 0, ctypes.byref(ov), _stream())
-    check(rc, "heal_v2v_aggregate")
+        _call("heal_v2v_aggregate", q.view(), p_node.view(), x.view(), _p(th), _host_i32(flat), U, H, W, C,
+              1 if agg_max else 0, 1 if gru else 0, out.view())
     return out
 
 
+@_guard
 def gru_gate(zc: Act, out: Optional[Act] = None, out_fmt: Optional[str] = None) -> Act:
     """Zero-hidden ConvGRU cell output: zc Act (N,H,W,2C) = (update-gate | candidate) conv output -> Act (N,H,W,C)
     = sigmoid(zc[..., :C]) * tanh(zc[..., C:])."""
     N, H, W = zc.N, zc.H, zc.W
     assert zc.C % 2 == 0
     C = zc.C // 2
-    if out is None:
-        out = act_empty(N, H, W, C, out_fmt or zc.fmt, zc.device)
-    assert (out.N, out.H, out.W, out.C) == (N, H, W, C)
-    zv, ov = zc.view(), out.view()
+    out = _out_act(out, N, H, W, C, out_fmt or zc.fmt, zc.device)
     npix = N * H * W
     with _Prof("gru_gate", 4.0 * npix * C, npix * float(C) * (2 * BPE[zc.fmt] + BPE[out.fmt])):
-        rc = lib.heal_gru_gate(ctypes.byref(zv), npix, C, ctypes.byref(ov), _stream())
-    check(rc, "heal_gru_gate")
+        _call("heal_gru_gate", zc.view(), npix, C, out.view())
     return out
 
 
+@_guard
 def swap_attention(qkv: Act, n_agents: Sequence[int], L: int, window_size: int, grid: bool, bias: torch.Tensor,
                    out: Optional[Act] = None, out_fmt: Optional[str] = None) -> Act:
     """CoBEVT window (grid False) or grid (grid True) attention core.  qkv Act (B*L,H,W,3C) = to_qkv output with q pre-scaled;
@@ -781,20 +811,17 @@ def swap_attention(qkv: Act, n_agents: Sequence[int], L: int, window_size: int, 
     n = L * window_size * window_size
     assert qkv.N == B * L and qkv.C == 3 * C and bias.dtype == torch.float32 and bias.is_contiguous()
     assert bias.shape == (C // 32, n, n)
-    if out is None:
-        out = act_empty(B * L, H, W, C, out_fmt or qkv.fmt, qkv.device)
-    assert (out.N, out.H, out.W, out.C) == (B * L, H, W, C)
+    out = _out_act(out, B * L, H, W, C, out_fmt or qkv.fmt, qkv.device)
     keys = float(sum(int(v) for v in n_agents)) * window_size * window_size     # valid keys per query, summed over scenes
     wins = (H // window_size) * (W // window_size)
-    qv, ov = qkv.view(), out.view()
     with _Prof("swap_attention", 4.0 * keys * C * wins * n,
                B * L * H * W * float(C) * (3 * BPE[qkv.fmt] + BPE[out.fmt])):
-        rc = lib.heal_swap_attention(ctypes.byref(qv), _host_i32(n_agents), B, L, H, W, C, int(window_size), 1 if grid else 0,
-                                     _p(bias), ctypes.byref(ov), _stream())
-    check(rc, "heal_swap_attention")
+        _call("heal_swap_attention", qkv.view(), _host_i32(n_agents), B, L, H, W, C, int(window_size), 1 if grid else 0,
+              _p(bias), out.view())
     return out
 
 
+@_guard
 def mean_layernorm(x: Act, n_avg: int, ln_weight: torch.Tensor, ln_bias: torch.Tensor, eps: float,
                    out: Optional[Act] = None, out_fmt: Optional[str] = None) -> Act:
     """x Act (N*n_avg,H,W,C) -> Act (N,H,W,C): LayerNorm over channels of the mean of every n_avg consecutive images
@@ -802,18 +829,14 @@ def mean_layernorm(x: Act, n_avg: int, ln_weight: torch.Tensor, ln_bias: torch.T
     _need_cuda(ln_weight, ln_bias)
     assert x.N % n_avg == 0
     N, H, W, C = x.N // n_avg, x.H, x.W, x.C
-    if out is None:
-        out = act_empty(N, H, W, C, out_fmt or x.fmt, x.device)
-    assert (out.N, out.H, out.W, out.C) == (N, H, W, C)
+    out = _out_act(out, N, H, W, C, out_fmt or x.fmt, x.device)
     lw, lb = ln_weight.float().contiguous(), ln_bias.float().contiguous()
-    xv, ov = x.view(), out.view()
     with _Prof("mean_layernorm", 0, N * H * W * float(C) * (n_avg * BPE[x.fmt] + BPE[out.fmt])):
-        rc = lib.heal_mean_layernorm(ctypes.byref(xv), N, int(n_avg), H, W, C, _p(lw), _p(lb), float(eps), ctypes.byref(ov),
-                                     _stream())
-    check(rc, "heal_mean_layernorm")
+        _call("heal_mean_layernorm", x.view(), N, int(n_avg), H, W, C, _p(lw), _p(lb), float(eps), out.view())
     return out
 
 
+@_guard
 def window_attention(qkv: Act, heads: int, dim_head: int, window_size: int, bias: torch.Tensor, qkv_coffset: int = 0,
                      out: Optional[Act] = None, out_coffset: int = 0, out_fmt: Optional[str] = None) -> Act:
     """One V2X-ViT window-attention branch.  qkv Act (N,H,W,>=3*heads*dim_head): q | k | v of the branch from channel
@@ -826,15 +849,14 @@ def window_attention(qkv: Act, heads: int, dim_head: int, window_size: int, bias
     if out is None:
         out = act_empty(N, H, W, inner, out_fmt or qkv.fmt, qkv.device)
     assert (out.N, out.H, out.W) == (N, H, W) and out_coffset + inner <= out.C
-    qv, ov = qkv.view(qkv_coffset), out.view(out_coffset)
     with _Prof("window_attention", 4.0 * N * H * W * n * inner,
                N * H * W * float(inner) * (3 * BPE[qkv.fmt] + BPE[out.fmt])):
-        rc = lib.heal_window_attention(ctypes.byref(qv), N, H, W, int(heads), int(dim_head), int(window_size), _p(bias),
-                                       ctypes.byref(ov), _stream())
-    check(rc, "heal_window_attention")
+        _call("heal_window_attention", qkv.view(qkv_coffset), N, H, W, int(heads), int(dim_head), int(window_size), _p(bias),
+              out.view(out_coffset))
     return out
 
 
+@_guard
 def cav_attention(qkv: Act, n_agents: Sequence[int], ego_only: bool, out: Optional[Act] = None,
                   out_fmt: Optional[str] = None) -> Act:
     """V2X-ViT per-pixel agent attention (HGTCavAttention with agent types 0).  qkv Act (N,H,W,3C), N = sum(n_agents), images
@@ -844,19 +866,15 @@ def cav_attention(qkv: Act, n_agents: Sequence[int], ego_only: bool, out: Option
     total = sum(int(v) for v in n_agents)
     assert qkv.N == total and qkv.C == 3 * C
     nq = B if ego_only else total
-    if out is None:
-        out = act_empty(nq, H, W, C, out_fmt or qkv.fmt, qkv.device)
-    assert (out.N, out.H, out.W, out.C) == (nq, H, W, C)
+    out = _out_act(out, nq, H, W, C, out_fmt or qkv.fmt, qkv.device)
     pairs = float(sum(int(v) for v in n_agents)) if ego_only else float(sum(int(v) ** 2 for v in n_agents))
-    qv, ov = qkv.view(), out.view()
     with _Prof("cav_attention", 4.0 * pairs * H * W * C, H * W * float(C) * (2 * total + nq) * BPE[qkv.fmt]
                + nq * H * W * float(C) * BPE[out.fmt]):
-        rc = lib.heal_cav_attention(ctypes.byref(qv), _host_i32(n_agents), B, H, W, C, 1 if ego_only else 0,
-                                    ctypes.byref(ov), _stream())
-    check(rc, "heal_cav_attention")
+        _call("heal_cav_attention", qkv.view(), _host_i32(n_agents), B, H, W, C, 1 if ego_only else 0, out.view())
     return out
 
 
+@_guard
 def split_attn(o: Act, x: Act, fc1_t: torch.Tensor, ln_weight: torch.Tensor, ln_bias: torch.Tensor, eps: float,
                fc2_t: torch.Tensor, out: Optional[Act] = None, out_fmt: Optional[str] = None) -> Act:
     """SplitAttn + residual.  o Act (N,H,W,3C) = the three branch outputs side by side, x Act (N,H,W,C) -> Act (N,H,W,C) =
@@ -866,40 +884,34 @@ def split_attn(o: Act, x: Act, fc1_t: torch.Tensor, ln_weight: torch.Tensor, ln_
     N, H, W, C = x.N, x.H, x.W, x.C
     assert (o.N, o.H, o.W, o.C) == (N, H, W, 3 * C)
     assert fc1_t.shape == (C, C) and fc2_t.shape == (C, 3 * C) and fc1_t.is_contiguous() and fc2_t.is_contiguous()
-    if out is None:
-        out = act_empty(N, H, W, C, out_fmt or x.fmt, x.device)
-    assert (out.N, out.H, out.W, out.C) == (N, H, W, C)
+    out = _out_act(out, N, H, W, C, out_fmt or x.fmt, x.device)
     lw, lb = ln_weight.float().contiguous(), ln_bias.float().contiguous()
     nbytes = int(lib.heal_split_attn_workspace(N, C))
     ws = _workspace(x.device, nbytes)
-    ov, xv, dv = o.view(), x.view(), out.view()
     with _Prof("split_attn", N * (2.0 * C * C * 4 + 6.0 * H * W * C),
                N * H * W * float(C) * (6 * BPE[o.fmt] + BPE[x.fmt] + BPE[out.fmt])):
-        rc = lib.heal_split_attn(ctypes.byref(ov), ctypes.byref(xv), N, H, W, C, _p(fc1_t), _p(lw), _p(lb), float(eps),
-                                 _p(fc2_t), _p(ws), ws.numel(), ctypes.byref(dv), _stream())
-    check(rc, "heal_split_attn")
+        _call("heal_split_attn", o.view(), x.view(), N, H, W, C, _p(fc1_t), _p(lw), _p(lb), float(eps),
+              _p(fc2_t), _p(ws), ws.numel(), out.view())
     return out
 
 
+@_guard
 def sttf_resample(src: Act, theta: torch.Tensor, out: Optional[Act] = None, out_fmt: Optional[str] = None) -> Act:
     """V2X-ViT STTF warp: out image k = grid_sample(src image k, affine_grid(theta[k])), bilinear, zeros, align_corners=True.
     theta (N,2,3) fp32 on the device."""
     _need_cuda(theta)
     N, H, W, C = src.N, src.H, src.W, src.C
     assert theta.dtype == torch.float32 and theta.is_contiguous() and theta.shape == (N, 2, 3)
-    if out is None:
-        out = act_empty(N, H, W, C, out_fmt or src.fmt, src.device)
-    assert (out.N, out.H, out.W, out.C) == (N, H, W, C)
-    sv, ov = src.view(), out.view()
+    out = _out_act(out, N, H, W, C, out_fmt or src.fmt, src.device)
     with _Prof("sttf_resample", 8.0 * N * C * H * W, N * (BPE[src.fmt] + BPE[out.fmt]) * float(C) * H * W):
-        rc = lib.heal_sttf_resample(ctypes.byref(sv), _p(theta), N, H, W, C, ctypes.byref(ov), _stream())
-    check(rc, "heal_sttf_resample")
+        _call("heal_sttf_resample", src.view(), _p(theta), N, H, W, C, out.view())
     return out
 
 
 # ------------------------------------------------------------------------------------------------
 # Lift-Splat-Shoot
 # ------------------------------------------------------------------------------------------------
+@_guard
 def lss_camera_matrices(rots, intrins, post_rots):
     """(…,3,3) f32 each -> (post_rots^-1, rots @ intrins^-1) as (BN,3,3) f32; one capturable launch (torch.inverse is not)."""
     _need_cuda(rots, intrins, post_rots)
@@ -907,10 +919,11 @@ def lss_camera_matrices(rots, intrins, post_rots):
     k = intrins.reshape(-1, 3, 3).contiguous().float()
     pr = post_rots.reshape(-1, 3, 3).contiguous().float()
     post_inv, combine = torch.empty_like(pr), torch.empty_like(r)
-    check(lib.heal_lss_camera_matrices(_p(r), _p(k), _p(pr), r.shape[0], _p(post_inv), _p(combine), _stream()), "heal_lss_camera_matrices")
+    _call("heal_lss_camera_matrices", _p(r), _p(k), _p(pr), r.shape[0], _p(post_inv), _p(combine))
     return post_inv, combine
 
 
+@_guard
 def lss_cell_index(frustum, post_rots_inv, post_trans, combine, trans, lower, dx, nx) -> torch.Tensor:
     """frustum (D,fH,fW,3); per-image 3x3 / 3-vectors (BN,...) -> int32 (BN,D,fH,fW) BEV cell or -1."""
     _need_cuda(frustum, post_rots_inv, post_trans, combine, trans)
@@ -918,14 +931,13 @@ def lss_cell_index(frustum, post_rots_inv, post_trans, combine, trans, lower, dx
     BN = post_trans.shape[0]
     cell = torch.empty((BN, D, fH, fW), dtype=torch.int32, device=frustum.device)
     with _Prof("lss_cell_index", 0, BN * D * fH * fW * 4.0 + D * fH * fW * 12.0):
-        rc = lib.heal_lss_cell_index(_p(frustum.contiguous().float()), D, fH, fW, _p(post_rots_inv.contiguous().float()),
-                                     _p(post_trans.contiguous().float()), _p(combine.contiguous().float()),
-                                     _p(trans.contiguous().float()), BN, _host_f32(lower), _host_f32(dx), _host_i32(nx),
-                                     _p(cell), _stream())
-    check(rc, "heal_lss_cell_index")
+        _call("heal_lss_cell_index", _p(frustum.contiguous().float()), D, fH, fW, _p(post_rots_inv.contiguous().float()),
+              _p(post_trans.contiguous().float()), _p(combine.contiguous().float()),
+              _p(trans.contiguous().float()), BN, _host_f32(lower), _host_f32(dx), _host_i32(nx), _p(cell))
     return cell
 
 
+@_guard
 def lss_pool(depth_logits, feat, cell, cams_per_agent: int, nx, ny) -> Act:
     """depth_logits (BN,D,fH,fW), feat (BN,C,fH,fW) f32 NCHW, cell (BN,D,fH,fW) -> Act f32 (agents, ny, nx, C)."""
     _need_cuda(depth_logits, feat, cell)
@@ -934,13 +946,13 @@ def lss_pool(depth_logits, feat, cell, cams_per_agent: int, nx, ny) -> Act:
     agents = BN // cams_per_agent
     with _Prof("lss_pool(+bev memset)", 2.0 * BN * D * fH * fW * C,
                BN * fH * fW * 4.0 * (2 * D + C) + agents * float(ny) * nx * C * 4):
-        out = torch.zeros((agents, ny, nx, C), dtype=torch.float32, device=feat.device)
-        rc = lib.heal_lss_pool(_p(depth_logits.contiguous().float()), _p(feat.contiguous().float()), _p(cell.contiguous()),
-                               BN, cams_per_agent, D, C, fH, fW, nx * ny, _p(out), _stream())
-    check(rc, "heal_lss_pool")
-    return Act(out, "f32")
+        out = act_zeros(agents, ny, nx, C, "f32", feat.device)
+        _call("heal_lss_pool", _p(depth_logits.contiguous().float()), _p(feat.contiguous().float()), _p(cell.contiguous()),
+              BN, cams_per_agent, D, C, fH, fW, nx * ny, _p(out.t))
+    return out
 
 
+@_guard
 def lss_pool_sorted(logits: torch.Tensor, l_strides, feat: torch.Tensor, f_strides, cell: torch.Tensor, cams_per_agent: int,
                     D: int, C: int, fH: int, fW: int, nx: int, ny: int, out_fmt: str = "f32") -> Act:
     """Deterministic LSS pooling (heal_lss_pool_sorted).  `logits` / `feat` are fp32 tensors whose data_ptr is the first logit /
@@ -950,17 +962,14 @@ def lss_pool_sorted(logits: torch.Tensor, l_strides, feat: torch.Tensor, f_strid
     assert logits.dtype == torch.float32 and feat.dtype == torch.float32 and cell.dtype == torch.int32 and cell.is_contiguous()
     BN = cell.shape[0]
     agents = BN // cams_per_agent
-    out = act_empty(agents, ny, nx, C, out_fmt, feat.device)
-    out.t.zero_()                                   # all-zero bits are 0.0 in every storage format; the kernel writes hit cells only
+    out = act_zeros(agents, ny, nx, C, out_fmt, feat.device)
     wsb = lib.heal_lss_pool_sorted_workspace(BN, D, fH, fW, agents, nx * ny)
     ws = _workspace(feat.device, wsb)
-    ov = out.view()
     npts = BN * D * fH * fW
     with _Prof("lss_pool_sorted", 2.0 * npts * C, BN * fH * fW * 4.0 * (2 * D + C) + agents * float(ny) * nx * C * BPE[out_fmt]):
-        rc = lib.heal_lss_pool_sorted(_p(logits), int(l_strides[0]), int(l_strides[1]), int(l_strides[2]),
-                                      _p(feat), int(f_strides[0]), int(f_strides[1]), int(f_strides[2]),
-                                      _p(cell), BN, cams_per_agent, D, C, fH, fW, nx * ny, ctypes.byref(ov), _p(ws), ws.numel(), _stream())
-    check(rc, "heal_lss_pool_sorted")
+        _call("heal_lss_pool_sorted", _p(logits), int(l_strides[0]), int(l_strides[1]), int(l_strides[2]),
+              _p(feat), int(f_strides[0]), int(f_strides[1]), int(f_strides[2]),
+              _p(cell), BN, cams_per_agent, D, C, fH, fW, nx * ny, out.view(), _p(ws), ws.numel())
     return out
 
 
@@ -990,33 +999,34 @@ class SparseTensor:
         return out
 
 
+@_guard
 def sp_build_table(st: SparseTensor):
     if st.table is None:
         ts = lib.heal_spconv_table_size(st.capacity)
         keys = torch.empty((ts,), dtype=torch.int32, device=st.coords.device)
         vals = torch.empty((ts,), dtype=torch.int32, device=st.coords.device)
         with _Prof("spconv_rulebook"):
-            rc = lib.heal_spconv_build_table(_p(st.coords), _p(st.rows_dev), st.capacity, _host_i32(st.spatial_shape), st.batch,
-                                             _p(keys), _p(vals), _stream())
-        check(rc, "heal_spconv_build_table")
+            _call("heal_spconv_build_table", _p(st.coords), _p(st.rows_dev), st.capacity, _host_i32(st.spatial_shape), st.batch,
+                  _p(keys), _p(vals))
         st.table = (keys, vals)
     return st.table
 
 
+@_guard
 def sp_subm_neighbors(st: SparseTensor, ksize) -> torch.Tensor:
     keys, vals = sp_build_table(st)
     K = int(ksize[0] * ksize[1] * ksize[2])
     nbr = torch.empty((st.capacity, K), dtype=torch.int32, device=st.coords.device)
     with _Prof("spconv_rulebook"):
-        rc = lib.heal_spconv_subm_neighbors(_p(st.coords), _p(st.rows_dev), st.capacity, _host_i32(st.spatial_shape),
-                                            _host_i32(ksize), _p(keys), _p(vals), st.table_capacity, _p(nbr), _stream())
-    check(rc, "heal_spconv_subm_neighbors")
+        _call("heal_spconv_subm_neighbors", _p(st.coords), _p(st.rows_dev), st.capacity, _host_i32(st.spatial_shape),
+              _host_i32(ksize), _p(keys), _p(vals), st.table_capacity, _p(nbr))
     return nbr
 
 
 SP_GROWTH = 2.0     # default output-row capacity of a strided sparse conv relative to its input capacity (see sp_strided)
 
 
+@_guard
 def sp_strided(st: SparseTensor, ksize, stride, pad, out_capacity: Optional[int] = None):
     """SparseConv3d rulebook: returns (output SparseTensor without feats, nbr (out_cap, K)).  No host sync: the live output
     row count stays on the device (`rows_dev`; rows beyond `out_capacity` are dropped by the kernels and show up as
@@ -1041,10 +1051,9 @@ def sp_strided(st: SparseTensor, ksize, stride, pad, out_capacity: Optional[int]
     wsb = lib.heal_spconv_strided_workspace(st.capacity, out_capacity, K)
     ws = _workspace(dev, wsb)
     with _Prof("spconv_rulebook"):
-        rc = lib.heal_spconv_strided_rulebook(_p(st.coords), _p(st.rows_dev), st.capacity, _host_i32(oshape), st.batch,
-                                              _host_i32(ksize), _host_i32(stride), _host_i32(pad), out_capacity,
-                                              _p(ocoords), _p(orows), _p(okeys), _p(ovals), _p(nbr), _p(ws), ws.numel(), _stream())
-    check(rc, "heal_spconv_strided_rulebook")
+        _call("heal_spconv_strided_rulebook", _p(st.coords), _p(st.rows_dev), st.capacity, _host_i32(oshape), st.batch,
+              _host_i32(ksize), _host_i32(stride), _host_i32(pad), out_capacity,
+              _p(ocoords), _p(orows), _p(okeys), _p(ovals), _p(nbr), _p(ws), ws.numel())
     return SparseTensor(None, ocoords, orows, oshape, st.batch, (okeys, ovals), table_capacity=out_capacity), nbr
 
 
@@ -1060,6 +1069,7 @@ def sp_check_overflow(tensors) -> None:
                                "raise heal_b200.ops.SP_GROWTH or pass out_capacity")
 
 
+@_guard
 def sp_gather_gemm(feats: torch.Tensor, nbr: torch.Tensor, rows_dev, weight: torch.Tensor, bias, relu: bool) -> torch.Tensor:
     """feats (Min,Cin) f32; nbr (cap,K) i32; weight (K,Cin,Cout) f32 (BN folded) -> (cap,Cout) f32."""
     _need_cuda(feats, nbr, weight)
@@ -1072,9 +1082,8 @@ def sp_gather_gemm(feats: torch.Tensor, nbr: torch.Tensor, rows_dev, weight: tor
         return float((nbr[:m] >= 0).sum().item()), float(m)
     with _Prof("spconv_gather_gemm", lambda: 2.0 * _pairs()[0] * cin * cout,
                lambda: _pairs()[0] * (cin * 4.0 + 4.0) + _pairs()[1] * (cout * 4.0 + K * 4.0)):
-        rc = lib.heal_spconv_gather_gemm(_p(feats), _p(nbr), _p(rows_dev), cap, K, _p(weight), _p(bias), cin, cout,
-                                         1 if relu else 0, _p(out), _stream())
-    check(rc, "heal_spconv_gather_gemm")
+        _call("heal_spconv_gather_gemm", _p(feats), _p(nbr), _p(rows_dev), cap, K, _p(weight), _p(bias), cin, cout,
+              1 if relu else 0, _p(out))
     return out
 
 
@@ -1093,16 +1102,17 @@ def pack_spconv_tc(wp: torch.Tensor) -> torch.Tensor:
     return split_bf16(rows.reshape(kb * cout, 64), 2).to(wp.device)
 
 
+@_guard
 def rows_to_split(feats: torch.Tensor, rows_dev) -> torch.Tensor:
     """(cap, C) fp32 rows -> (cap, 2C) bf16 split rows [hi | lo]."""
     cap, C = feats.shape
     out = torch.empty((cap, 2 * C), dtype=torch.bfloat16, device=feats.device)
     with _Prof("rows_to_split", 0, cap * C * 8.0):
-        rc = lib.heal_rows_to_split(_p(feats), _p(rows_dev), cap, C, _p(out), _stream())
-    check(rc, "heal_rows_to_split")
+        _call("heal_rows_to_split", _p(feats), _p(rows_dev), cap, C, _p(out))
     return out
 
 
+@_guard
 def sp_gather_gemm_tc(feats_split: torch.Tensor, nbr: torch.Tensor, rows_dev, w_packed: torch.Tensor, bias, relu: bool,
                       cin: int, cout: int, want_f32: bool = False) -> torch.Tensor:
     """feats_split (Min, 2*Cin) bf16 split rows; nbr (cap,K) i32 -> (cap, 2*Cout) bf16 split rows, or (cap, Cout) fp32."""
@@ -1117,22 +1127,20 @@ def sp_gather_gemm_tc(feats_split: torch.Tensor, nbr: torch.Tensor, rows_dev, w_
         return float((nbr[:m] >= 0).sum().item()), float(m)
     with _Prof("spconv_gather_gemm_tc", lambda: 2.0 * _pairs()[0] * cin * cout,
                lambda: _pairs()[0] * (cin * 4.0 + 4.0) + _pairs()[1] * (cout * 4.0 + K * 4.0)):
-        rc = lib.heal_spconv_gather_gemm_tc(_p(feats_split), _p(nbr), _p(rows_dev), cap, K, _p(w_packed), _p(bias), cin, cout,
-                                            1 if relu else 0, _vp(0) if want_f32 else _p(out), _p(out) if want_f32 else _vp(0),
-                                            0, 0, 0, 0, _stream())
-    check(rc, "heal_spconv_gather_gemm_tc")
+        _call("heal_spconv_gather_gemm_tc", _p(feats_split), _p(nbr), _p(rows_dev), cap, K, _p(w_packed), _p(bias), cin, cout,
+              1 if relu else 0, _vp(0) if want_f32 else _p(out), _p(out) if want_f32 else _vp(0), 0, 0, 0, 0)
     return out
 
 
+@_guard
 def sparse_to_bev(st: SparseTensor) -> Act:
     """HeightCompression: (B, H, W, C*D) channels-last fp32 with channel = c*D + z."""
     D, H, W = st.spatial_shape
     C = st.feats.shape[1]
     with _Prof("sparse_to_bev(+memset)", 0, st.batch * float(H) * W * C * D * 4 + st.capacity * (C * 4.0 + 16)):
-        out = torch.zeros((st.batch, H, W, C * D), dtype=torch.float32, device=st.feats.device)
-        rc = lib.heal_sparse_to_bev(_p(st.feats), _p(st.coords), _p(st.rows_dev), st.capacity, C, D, H, W, _p(out), _stream())
-    check(rc, "heal_sparse_to_bev")
-    return Act(out, "f32")
+        out = act_zeros(st.batch, H, W, C * D, "f32", st.feats.device)
+        _call("heal_sparse_to_bev", _p(st.feats), _p(st.coords), _p(st.rows_dev), st.capacity, C, D, H, W, _p(out.t))
+    return out
 
 
 # ------------------------------------------------------------------------------------------------
@@ -1156,6 +1164,7 @@ class SparseCanvas:
         return self._densify(fmt)
 
 
+@_guard
 def pillar_vfe_sparse(voxel_features, voxel_num_points, voxel_coords, w_folded, b_folded, voxel_size, lidar_range,
                       nx: int, ny: int, batch_size: int, num_voxels_dev: Optional[torch.Tensor] = None,
                       want_split_rows: bool = False) -> SparseCanvas:
@@ -1168,8 +1177,7 @@ def pillar_vfe_sparse(voxel_features, voxel_num_points, voxel_coords, w_folded, 
     coords = voxel_coords.to(torch.int32).contiguous()
     idmap = torch.empty((batch_size, ny, nx), dtype=torch.int32, device=pf.device)
     with _Prof("pillar_idmap", 0, batch_size * float(ny) * nx * 4 + coords.shape[0] * 16.0):
-        rc = lib.heal_pillar_idmap(_p(coords), _p(num_voxels_dev), coords.shape[0], batch_size, ny, nx, _p(idmap), _stream())
-    check(rc, "heal_pillar_idmap")
+        _call("heal_pillar_idmap", _p(coords), _p(num_voxels_dev), coords.shape[0], batch_size, ny, nx, _p(idmap))
 
     def densify(fmt):
         _, canvas = pillar_vfe_scatter(voxel_features, voxel_num_points, voxel_coords, w_folded, b_folded, voxel_size,
@@ -1200,20 +1208,20 @@ def _sparse_stem_gather_tc(sc: SparseCanvas, pc_conv: PackedConv, pc_down: Packe
     nbr9 = torch.empty((rows, 9), dtype=torch.int32, device=dev)
     nbr1 = torch.empty((rows, 1), dtype=torch.int32, device=dev)
     with _Prof("sparse_stem_rulebook", 0, rows * 40.0 + B * float(sc.H) * sc.W * 4):
-        check(lib.heal_stem_rulebook(_p(sc.idmap), B, sc.H, sc.W, 3, 1, _p(nbr9), _stream()), "heal_stem_rulebook")
-        check(lib.heal_stem_rulebook(_p(sc.idmap), B, sc.H, sc.W, 1, 0, _p(nbr1), _stream()), "heal_stem_rulebook")
+        _call("heal_stem_rulebook", _p(sc.idmap), B, sc.H, sc.W, 3, 1, _p(nbr9))
+        _call("heal_stem_rulebook", _p(sc.idmap), B, sc.H, sc.W, 1, 0, _p(nbr1))
 
     def _hits():
         return float((sc.idmap >= 0).sum().item())
     with _Prof("sparse_stem_tc", lambda: 2.0 * 64 * 64 * (2.25 + 0.25) * _hits(),
                lambda: rows * 40.0 + _hits() * 2.5 * 256.0 + 2.0 * rows * 64 * 4):
         for nbr, pc, o, relu in ((nbr9, pc_conv, o1, 1), (nbr1, pc_down, o2, 0)):
-            rc = lib.heal_spconv_gather_gemm_tc(_p(sc.feats_split), _p(nbr), _vp(0), rows, nbr.shape[1], _p(pc._sp_packed), _p(pc.bias), 64, 64,
-                                                relu, _p(o.t), _vp(0), 0, 0, o.cstride, o.plane_stride, _stream())
-            check(rc, "heal_spconv_gather_gemm_tc")
+            _call("heal_spconv_gather_gemm_tc", _p(sc.feats_split), _p(nbr), _vp(0), rows, nbr.shape[1], _p(pc._sp_packed),
+                  _p(pc.bias), 64, 64, relu, _p(o.t), _vp(0), 0, 0, o.cstride, o.plane_stride)
     return o1, o2
 
 
+@_guard
 def sparse_stem(sc: SparseCanvas, pc_conv: PackedConv, pc_down: PackedConv, out_fmt: str, tensor_cores: bool = False):
     """BasicBlock.conv1(3x3 s2 p1)+bn1+ReLU and downsample(1x1 s2)+bn from the pillar list. Returns (Act conv, Act down).
     tensor_cores: split-bf16 mma.sync variant (fp32-equivalent; the tc32 / bf16 engine modes), else fp32 FMAs."""
@@ -1223,16 +1231,14 @@ def sparse_stem(sc: SparseCanvas, pc_conv: PackedConv, pc_down: PackedConv, out_
     o2 = act_empty(sc.N, sc.H // 2, sc.W // 2, 64, out_fmt, sc.device)
     if STEM_GATHER_TC and out_fmt == "split" and sc.feats_split is not None:
         return _sparse_stem_gather_tc(sc, pc_conv, pc_down, o1, o2)
-    v1, v2 = o1.view(), o2.view()
-    fn = lib.heal_sparse_stem_tc if (tensor_cores and sc.W % 32 == 0) else lib.heal_sparse_stem
+    symbol = "heal_sparse_stem_tc" if (tensor_cores and sc.W % 32 == 0) else "heal_sparse_stem"
     def _stem():
         hits = float((sc.idmap >= 0).sum().item())
         return hits
     with _Prof("sparse_stem", lambda: 2.0 * 64 * 64 * (2.25 + 0.25) * _stem(),
                lambda: sc.N * float(sc.H) * sc.W * 4 + _stem() * 256.0 + 2.0 * sc.N * (sc.H // 2) * (sc.W // 2) * 64 * BPE[out_fmt]):
-        rc = fn(_p(sc.feats), _p(sc.idmap), sc.N, sc.H, sc.W, _p(pc_conv.weight), _p(pc_conv.bias),
-                _p(pc_down.weight), _p(pc_down.bias), 64, ctypes.byref(v1), ctypes.byref(v2), _stream())
-    check(rc, "heal_sparse_stem")
+        _call(symbol, _p(sc.feats), _p(sc.idmap), sc.N, sc.H, sc.W, _p(pc_conv.weight), _p(pc_conv.bias),
+              _p(pc_down.weight), _p(pc_down.bias), 64, o1.view(), o2.view())
     return o1, o2
 
 
@@ -1262,6 +1268,7 @@ def _head_act(t) -> Act:
     return to_act(t)
 
 
+@_guard
 def box_decode_nms(cls_preds, reg_preds, dir_preds, anchors: torch.Tensor, transform, score_threshold: float, nms_threshold: float,
                    dir_offset: float = 0.0, num_bins: int = 2, order: str = "hwl", gt_range=None, top: int = 1000,
                    buffers: Optional[PostprocessBuffers] = None) -> PostprocessBuffers:
@@ -1278,61 +1285,21 @@ def box_decode_nms(cls_preds, reg_preds, dir_preds, anchors: torch.Tensor, trans
     assert (buffers.H, buffers.W, buffers.A, buffers.top) == (H, W, A, top)
     T = _host_f32(np.asarray(torch.as_tensor(transform).detach().cpu().numpy(), dtype=np.float64).reshape(16))
     rng = _host_f32(gt_range) if gt_range is not None else None
-    cv, rv = c.view(), r.view()
-    dv = d.view() if d is not None else None
     with _Prof("box_decode_nms", 0):
-        rc = lib.heal_box_decode_nms(ctypes.byref(cv), ctypes.byref(rv), ctypes.byref(dv) if dv is not None else None, _p(anchors),
-                                     H, W, A, float(score_threshold), float(np.float32(dir_offset)), int(num_bins), T,
-                                     1 if order == "hwl" else 0, float(nms_threshold), int(top), rng,
-                                     _p(buffers.boxes), _p(buffers.scores), _p(buffers.count), _p(buffers.stats),
-                                     _p(buffers.workspace), buffers.workspace.numel(), _stream())
-    check(rc, "heal_box_decode_nms")
+        _call("heal_box_decode_nms", c.view(), r.view(), d.view() if d is not None else None, _p(anchors),
+              H, W, A, float(score_threshold), float(np.float32(dir_offset)), int(num_bins), T,
+              1 if order == "hwl" else 0, float(nms_threshold), int(top), rng,
+              _p(buffers.boxes), _p(buffers.scores), _p(buffers.count), _p(buffers.stats),
+              _p(buffers.workspace), buffers.workspace.numel())
     return buffers
 
 
-# ------------------------------------------------------------------------------------------------
-# device guard: the library launches on the CURRENT device and on the stream passed in; every public wrapper therefore runs
-# with its tensors' device made current (a model on cuda:1 while cuda:0 is current, or one process driving two GPUs).
-# ------------------------------------------------------------------------------------------------
-import functools as _functools
+def _first_cav_anchors(cavs, *args, **kwargs):
+    """box_decode_nms_multi's device argument: the first cav's anchors (the heads may be Acts or tensors)."""
+    return cavs[0]["anchors"] if cavs else None
 
 
-def _device_of(x):
-    if isinstance(x, torch.Tensor):
-        return x.device if x.is_cuda else None
-    if isinstance(x, (Act, SparseCanvas)):
-        return x.device
-    if isinstance(x, SparseTensor):
-        return x.coords.device
-    return None
-
-
-def _guard(fn):
-    @_functools.wraps(fn)
-    def wrapped(*args, **kwargs):
-        dev = None
-        for a in args:
-            dev = _device_of(a)
-            if dev is not None:
-                break
-        if dev is None:
-            for a in kwargs.values():
-                dev = _device_of(a)
-                if dev is not None:
-                    break
-        if dev is None or dev.index is None or dev.index == torch.cuda.current_device():
-            return fn(*args, **kwargs)
-        with torch.cuda.device(dev):
-            return fn(*args, **kwargs)
-    return wrapped
-
-
-for _name in ("mask_points", "dwconv_layernorm", "maxpool3x3s2", "convert", "voxelize", "mean_vfe", "pillar_vfe_scatter", "pillar_scatter", "conv2d_simt", "conv2d_tc", "pyramid_fuse_level", "att_fuse",
-              "lss_camera_matrices", "lss_cell_index", "lss_pool", "lss_pool_sorted", "sp_build_table", "sp_subm_neighbors", "sp_strided", "sp_gather_gemm", "sp_gather_gemm_tc", "rows_to_split", "sparse_to_bev",
-              "pillar_vfe_sparse", "sparse_stem", "box_decode_nms"):
-    globals()[_name] = _guard(globals()[_name])
-
-
+@_guard(device_arg=_first_cav_anchors)
 def box_decode_nms_multi(cavs, score_threshold: float, nms_threshold: float, dir_offset: float = 0.0, num_bins: int = 2,
                          order: str = "hwl", gt_range=None, top: int = 1000, buffers: Optional[PostprocessBuffers] = None) -> PostprocessBuffers:
     """VoxelPostprocessor.post_process for SEVERAL cavs (late fusion) and / or `iou_preds` rescoring on the GPU, no host sync.
@@ -1367,12 +1334,8 @@ def box_decode_nms_multi(cavs, score_threshold: float, nms_threshold: float, dir
     assert (buffers.H, buffers.W, buffers.A, buffers.top) == (H * n, W, A, top)
     rng = _host_f32(gt_range) if gt_range is not None else None
     with _Prof("box_decode_nms", 0):
-        rc = lib.heal_box_decode_nms_multi(arr, n, H, W, A, float(score_threshold), float(np.float32(dir_offset)), int(num_bins),
-                                           1 if order == "hwl" else 0, float(nms_threshold), int(top), rng,
-                                           _p(buffers.boxes), _p(buffers.scores), _p(buffers.count), _p(buffers.stats),
-                                           _p(buffers.workspace), buffers.workspace.numel(), _stream())
-    check(rc, "heal_box_decode_nms_multi")
+        _call("heal_box_decode_nms_multi", arr, n, H, W, A, float(score_threshold), float(np.float32(dir_offset)), int(num_bins),
+              1 if order == "hwl" else 0, float(nms_threshold), int(top), rng,
+              _p(buffers.boxes), _p(buffers.scores), _p(buffers.count), _p(buffers.stats),
+              _p(buffers.workspace), buffers.workspace.numel())
     return buffers
-
-
-box_decode_nms_multi = _guard(box_decode_nms_multi)

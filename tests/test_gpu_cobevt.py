@@ -207,3 +207,20 @@ def test_cobevt_graph_replay_is_bit_identical(golden_dir):
         graph.replay()
         torch.cuda.synchronize()
         assert torch.equal(ops.act_to_nchw(out), eager)
+
+
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two CUDA devices")
+def test_cobevt_on_a_device_that_is_not_current(golden_dir):
+    """The library launches on the current device, so every ops wrapper makes its inputs' device current: CoBEVT on cuda:1
+    run with cuda:0 current gives the bits it gives with cuda:1 current."""
+    from heal_b200 import engine
+    engine.set_precision("tc32")
+    g = cb.load_module_golden(golden_dir)["c64"]
+    x, rl, _ = cb.case_inputs("c64")
+    m = _loaded(g["args"], g["shapes"]).to("cuda:1")
+    x1, aff1 = x.to("cuda:1"), g["affine"].to("cuda:1")
+    outs = []
+    for current in (1, 0):
+        with torch.cuda.device(current), torch.no_grad():
+            outs.append(m(x1, rl, aff1).cpu())
+    assert torch.equal(outs[0], outs[1])

@@ -53,8 +53,12 @@ the output was exact)
   v2v      split_mean_gru 0.140, bf16_max_gru 0.086, f32_mean 0.127, split_max 0.100
   gru      split 0.243, bf16 0.208, f32 0.248
 so ALPHA = 2^-20 leaves 4x of headroom over the largest (gru_f32)."""
+import json
 import math
+import os
 import re
+import subprocess
+import sys
 import zlib
 from dataclasses import dataclass
 from typing import Optional, Tuple
@@ -624,38 +628,59 @@ _KERNEL = re.compile(r"\b(k_(?:pyramid_fuse_split8|pyramid_fuse|att_fuse_split8|
                      r"\b(?:<\s*(?:\(int\))?\s*(\d+)\s*>)?")
 
 
+def _launched_name(key):
+    """`k_name<N>` for a fuse.cu kernel's profiler name, None for any other kernel (torch's fills and copies)."""
+    m = _KERNEL.search(key)
+    return m.group(1) + (f"<{m.group(2)}>" if m.group(2) else "") if m else None
+
+
 def _launched(prof):
-    out = set()
-    for e in prof.key_averages():
-        m = _KERNEL.search(e.key)
-        if m:
-            out.add(m.group(1) + (f"<{m.group(2)}>" if m.group(2) else ""))
-    return out
+    return {n for n in (_launched_name(e.key) for e in prof.key_averages()) if n}
+
+
+def _profiled_kernels():
+    """Runs every case under one torch.profiler session and returns the fuse.cu kernels it recorded, in launch order (each case is
+    two library launches, runs A and B, so the list holds the cases' pairs in case order).  A session that recorded none of the
+    launches the library counted is repeated once (a wrong kernel never is)."""
+    from torch.autograd import DeviceType
+    from torch.profiler import ProfilerActivity, profile
+    from heal_b200._lib import lib
+    for _ in range(2):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for case in CASES:
+                before = lib.heal_launch_count()
+                _launch(case)
+                torch.cuda.synchronize()
+                assert lib.heal_launch_count() - before == 2, f"{case.name}: runs A and B are one launch each"
+        ours = sorted((e.time_range.start, _launched_name(e.name)) for e in prof.events()
+                      if e.device_type == DeviceType.CUDA and _launched_name(e.name))
+        if ours:
+            break
+    return [n for _, n in ours]
 
 
 @pytest.mark.gpu
-def test_cases_reach_every_instantiation():
+def test_each_case_launches_its_instantiations():
     """Each case runs the instantiations its row names (kernel names from torch.profiler), and together the cases run all of
-    REACHABLE: a change to a dispatch predicate cannot quietly move a case off what it exists to test."""
-    from torch.profiler import ProfilerActivity, profile
-    from heal_b200._lib import lib
-    seen_all = set()
-    for case in CASES:
-        # torch.profiler can lose every kernel record of a short session late in a long process; a session that recorded none
-        # of the launches the library counted is repeated once (a wrong kernel is never retried)
-        for _ in range(2):
-            before = lib.heal_launch_count()
-            with profile(activities=[ProfilerActivity.CUDA]) as prof:
-                _launch(case)
-                torch.cuda.synchronize()
-            seen = _launched(prof)
-            assert lib.heal_launch_count() - before == 2, f"{case.name}: runs A and B are one launch each"
-            if seen:
-                break
-        assert seen == set(case.reaches), f"{case.name}: ran {sorted(seen)}, expected {sorted(case.reaches)}"
-        seen_all |= seen
-    print(f"instantiations reached: {len(seen_all & REACHABLE)} of {len(REACHABLE)}")
-    assert seen_all == REACHABLE
+    REACHABLE: a change to a dispatch predicate cannot quietly move a case off what it exists to test.
+
+    The profiler session runs in a child process.  torch.profiler's CUDA records travel through activity buffers that live for
+    the whole process, so a short session late in a long process can come back without any kernel record, depending on every
+    session and CUDA call the process made before it.  In a process of its own the session does not depend on what ran
+    earlier in the suite."""
+    tests_dir = os.path.dirname(os.path.abspath(__file__))
+    code = ("import json, sys; sys.path[:0] = [%r, %r]; import test_gpu_fuse_kernels as t; "
+            "print('KERNELS ' + json.dumps(t._profiled_kernels()))" % (tests_dir, os.path.dirname(tests_dir)))
+    r = subprocess.run([sys.executable, "-s", "-c", code], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True,
+                       timeout=600)
+    assert r.returncode == 0, r.stdout[-4000:]
+    names = json.loads([ln for ln in r.stdout.splitlines() if ln.startswith("KERNELS ")][-1][len("KERNELS "):])
+    assert len(names) == 2 * len(CASES), f"the session recorded {len(names)} fuse.cu kernels for {2 * len(CASES)} launches"
+    for i, case in enumerate(CASES):
+        assert set(names[2 * i:2 * i + 2]) == set(case.reaches), \
+            f"{case.name}: ran {names[2 * i:2 * i + 2]}, expected {sorted(case.reaches)}"
+    print(f"instantiations reached: {len(set(names) & REACHABLE)} of {len(REACHABLE)}")
+    assert set(names) == REACHABLE
 
 
 def _misaligned_call(kernel, where, fmt):
