@@ -24,8 +24,10 @@
 // chunk (fp32 / transposed-conv / narrow outputs are stored from the fragment straight to global memory).
 // The producer keeps STAGES k-blocks in flight, so the next tile's operands arrive while the consumers run the epilogue.
 // Modes: stride 2 through TMA element strides; grouped 3x3 as 16-channel sub-block MMAs on block-diagonal 64-channel
-// tiles; "halo" (3x3, stride 1, one-row tiles, N = 64): one activation box of TW+2 pixels per kernel ROW, the three
-// horizontal taps are row-shifted descriptors of the same smem tile (3x less L2->smem activation traffic).
+// tiles; "halo" (3x3, stride 1, N = 64, one-row tiles or grouped two-row tiles): one activation box of TH rows x TW+2 pixels per
+// kernel ROW, the three horizontal taps are row-shifted descriptors of the same smem tile (3x less L2->smem activation traffic);
+// "A-row ring" (3x3, stride 1, N = 128, one-row tiles): the same row reuse with the A rows in a ring of their own and weight-only
+// stages, K ordered (channel block, kernel row, kernel column).
 // HEAL_TC_* environment switches are measurement hooks (profiles/tc_experiment.py), not product paths.
 #include <cuda.h>
 #include <stdlib.h>
@@ -58,7 +60,9 @@ struct TcP {
     int up;                       // transposed conv (k == stride == up): n-tile -> (i,j) sub-position
     int pdl;                      // launched with programmatic stream serialization
     int bo_mode;                  // experiment: base-offset convention of the halo descriptors
-    int halo;                     // 3x3 stride-1, one-row tiles: ONE activation load per kernel ROW (TW+2 pixels) serves the 3 horizontal taps
+    int halo;                     // 3x3 stride-1, TH <= 2: ONE activation load per kernel ROW (TH x (TW+2) pixels) serves the 3 horizontal taps
+    int arow;                     // dense 3x3 stride-1, BLOCK_N = 128, TH == 1: K order (channel block, kernel row, kernel column); one
+                                  // A row of TW+2 pixels per (channel block, kernel row) in a ring of 2 serves the 3 columns' k-blocks
     int tma_out;                  // epilogue drains through shared memory + TMA tensor store (tmO valid)
     int res_tma;                  // STG >= 2: the residual chunk is TMA-loaded into the staging buffer one chunk ahead (tmR valid)
     int dbg;                      // HEAL_TC_DBG experiment bits (timing only, results invalid): 1 no stores, 2 no B loads, 4 no A loads, 8 no residual loads (TMA-store epilogue), 16 no MMAs
@@ -92,16 +96,20 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     if (smem_u32(smem) & 1023u) __trap();
     // weight bytes per (tap, plane) in a stage: a BLOCK_N x 64 tile, or (grouped, packed) the four 16x16 diagonal sub-blocks
     const int B_TILE_BYTES = p.bdiag ? (BLOCK_N / 16) * 512 : BLOCK_N * BLOCK_K * 2;
-    // halo mode: A = [plane][TW+2 rows][128 B] (padded to 1 KiB), B = [plane][3 taps][BLOCK_N rows][128 B]
-    const int halo_a_plane = (p.TW + 2) * 128;
+    // halo mode: A = [plane][TH][TW+2 rows][128 B] (padded to 1 KiB), B = [plane][3 taps][BLOCK_N rows][128 B]
+    const int halo_a_plane = p.TH * (p.TW + 2) * 128;
     const int halo_a_bytes = (p.planes * halo_a_plane + 1023) & ~1023;
-    const int stage_bytes = p.halo ? (halo_a_bytes + p.wplanes * 3 * B_TILE_BYTES) : (p.planes * A_TILE_BYTES + p.wplanes * B_TILE_BYTES);
+    // A-row ring mode: the stages hold B only; the A rows (halo layout, TH == 1) sit in a ring of 2 after the staging buffers
+    const int stage_bytes = p.halo ? (halo_a_bytes + p.wplanes * 3 * B_TILE_BYTES)
+                          : p.arow ? p.wplanes * B_TILE_BYTES : (p.planes * A_TILE_BYTES + p.wplanes * B_TILE_BYTES);
     const int stg_bytes = p.planes * A_TILE_BYTES;                        // one staging buffer: [plane][128 rows][128 B]
     uint8_t* stg = smem + (size_t)STAGES * stage_bytes;                   // 1024-aligned (stage_bytes is a multiple of 1024)
-    uint64_t* bars = reinterpret_cast<uint64_t*>(stg + (size_t)STG * stg_bytes);
-    // bars: full[STAGES], empty[STAGES], residual_full[3]
+    uint8_t* aring = stg + (size_t)STG * stg_bytes;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(aring + (p.arow ? 2 * halo_a_bytes : 0));
+    // bars: full[STAGES], empty[STAGES], residual_full[3], a_full[2], a_empty[2]
     const uint32_t bar_res = smem_u32(bars + 2 * STAGES);
-    const uint32_t smem_base = smem_u32(smem);
+    const uint32_t bar_afull = smem_u32(bars + 2 * STAGES + 3), bar_aempty = smem_u32(bars + 2 * STAGES + 5);
+    const uint32_t smem_base = smem_u32(smem), aring_base = smem_u32(aring);
     const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + STAGES);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -116,6 +124,7 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 8); }   // 8 consumer warps
         for (int a = 0; a < 3; ++a) mbar_init(bar_res + 8 * a, 1);
+        for (int a = 0; a < 2; ++a) { mbar_init(bar_afull + 8 * a, 1); mbar_init(bar_aempty + 8 * a, 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -136,17 +145,41 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         // ============================== TMA producer: warp 0 (whole warp loops, one elected lane issues) ==
         if (warp == 0) {
             int stage = 0; uint32_t phase = 0;
+            int ast = 0; uint32_t aphase = 0;
             for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
                 const int nt = tile % p.n_tiles, mt = tile / p.n_tiles;
                 const int tw_i = mt % p.tiles_w; const int t2 = mt / p.tiles_w;
                 const int th_i = t2 % p.tiles_h; const int img = t2 / p.tiles_h;
                 const int h0 = th_i * p.TH, w0 = tw_i * p.TW;
                 for (int kb = 0; kb < kblocks; ++kb) {
+                    if (p.arow) {
+                        // k-block = (channel block, kernel row r, kernel column s): at s == 0 the TW+2 pixels of input row h0+r-1
+                        // go to the A ring, then every k-block brings its tap's weight tile
+                        const int kc = kb / 9, tap = kb % 9, r = tap / 3, s = tap % 3;
+                        if (s == 0) {
+                            mbar_wait(bar_aempty + 8 * ast, aphase ^ 1);
+                            if (elect_one()) {
+                                mbar_expect_tx(bar_afull + 8 * ast, (uint32_t)(p.planes * halo_a_plane));
+                                tma_load_5d(aring_base + ast * halo_a_bytes, &tmA, bar_afull + 8 * ast, kc * BLOCK_K, w0 - 1, h0 + r - 1, img, 0);
+                            }
+                            __syncwarp();
+                        }
+                        mbar_wait(bar_empty + 8 * stage, phase ^ 1);
+                        if (elect_one()) {
+                            mbar_expect_tx(bar_full + 8 * stage, (uint32_t)(p.wplanes * B_TILE_BYTES));
+                            tma_load_3d(smem_base + stage * stage_bytes, &tmB, bar_full + 8 * stage, kc * BLOCK_K, tap * p.coutp + nt * BLOCK_N, 0);
+                        }
+                        __syncwarp();
+                        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+                        if (s == 2 && ++ast == 2) { ast = 0; aphase ^= 1; }
+                        continue;
+                    }
                     const int tap = kb / kcn, kc = p.blockdiag ? nt : kb % kcn;
                     const int r = tap / p.taps_w, s = tap % p.taps_w;
                     mbar_wait(bar_empty + 8 * stage, phase ^ 1);
                     if (p.halo) {
-                        // k-block = (kernel row tap, channel block): pixels [w0-1, w0+TW] of input row h0+tap-1, and the 3 taps' weights
+                        // k-block = (kernel row tap, channel block): pixels [w0-1, w0+TW] of input rows [h0+tap-1, h0+tap-1+TH), and the
+                        // 3 taps' weights
                         const uint32_t sa = smem_base + stage * stage_bytes, sb = sa + halo_a_bytes;
                         if (elect_one()) {
                             mbar_expect_tx(bar_full + 8 * stage, (uint32_t)(p.planes * halo_a_plane + p.wplanes * 3 * B_TILE_BYTES));
@@ -188,9 +221,13 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         const bool split = (p.planes == 2);                      // activations carry a lo plane
         const bool wsplit = (p.wplanes == 2);                    // weights carry a lo plane
         const int sub_bytes = p.wplanes * 2048;                  // smem bytes per 16-channel diagonal sub-block: [plane][16 rows][128 B]
-        const uint32_t a_plane = p.halo ? (uint32_t)halo_a_plane : (uint32_t)A_TILE_BYTES;
+        const uint32_t a_plane = (p.halo || p.arow) ? (uint32_t)halo_a_plane : (uint32_t)A_TILE_BYTES;
         const int ntap = p.halo ? 3 : 1;
+        // first A row of this warpgroup's 64 pixels: tile pixel 64 wg, i.e. tile row 64 wg / TW, column 64 wg % TW; a halo tile's
+        // rows are TW + 2 pixels long (TH == 2: warpgroup wg owns tile row wg)
+        const uint32_t a_row0 = (p.halo || p.arow) ? (uint32_t)((64 * wg / p.TW) * (p.TW + 2) + (64 * wg) % p.TW) : (uint32_t)(64 * wg);
         int stage = 0; uint32_t phase = 0;
+        int ast = 0; uint32_t aphase = 0;                       // A-row ring slot and parity (p.arow)
         float d[NACC / 2];
         float e[NCAT ? BLOCK_N / 2 : 1];                        // NCAT: a_lo*b_hi, or a_hi*b_hi with one weight plane
 #pragma unroll
@@ -202,16 +239,21 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         // N = BLOCK_N ones write e, not the first half of d): in-flight MMAs of different N on overlapping registers make ptxas
         // serialise the whole wgmma chain.
         auto mma_tile = [&]() {
-            int prev = -1;
+            int prev = -1, prev_a = -1;
             for (int kb = 0; kb < kblocks; ++kb) {
+                // A-row ring: kernel column tc of the row in ring slot ast (waited for at its first column)
+                const int tc = p.arow ? kb % 3 : 0;
+                if (p.arow && tc == 0) mbar_wait(bar_afull + 8 * ast, aphase);
                 mbar_wait(bar_full + 8 * stage, phase);
-                // A: [plane][rows][128 B]; halo mode: tap s reads rows [s, s+128) of the (TW+2)-row tile (start address + s*128 B)
-                const uint32_t sa = smem_base + stage * stage_bytes;
-                const uint32_t sb = sa + (p.halo ? (uint32_t)halo_a_bytes : (uint32_t)(p.planes * A_TILE_BYTES));
+                // A: [plane][rows][128 B]; halo mode: tap s reads rows [a_row0 + s, a_row0 + s + 64) of the TH x (TW+2)-row tile
+                // (start address + s*128 B); A-row ring: the same with s = tc, in the ring slot; B alone fills the stage
+                const uint32_t sa = p.arow ? aring_base + ast * halo_a_bytes + tc * 128 : smem_base + stage * stage_bytes;
+                const uint32_t sb = p.arow ? smem_base + stage * stage_bytes
+                                           : sa + (p.halo ? (uint32_t)halo_a_bytes : (uint32_t)(p.planes * A_TILE_BYTES));
                 wgmma_fence();
                 if (!(p.dbg & 16))
                 for (int s = 0; s < ntap; ++s) {
-                    const uint32_t ah = sa + (uint32_t)(wg * 64 * 128 + s * 128), al = ah + a_plane;
+                    const uint32_t ah = sa + (a_row0 + (uint32_t)s) * 128u, al = ah + a_plane;
                     const uint32_t bs = sb + s * p.wplanes * B_TILE_BYTES;
 #pragma unroll
                     for (int k = 0; k < BLOCK_K / 16; ++k) {
@@ -253,11 +295,18 @@ k_conv2d_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                 wgmma_commit();
                 wgmma_wait<1>();                                   // the previous k-block's MMAs have retired: free its stage
                 if (prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev);
+                if (prev_a >= 0 && lane == 0) mbar_arrive(bar_aempty + 8 * prev_a);   // the row's last column has retired
                 prev = stage;
+                prev_a = -1;
                 if (++stage == STAGES) { stage = 0; phase ^= 1; }
+                if (tc == 2) {
+                    prev_a = ast;
+                    if (++ast == 2) { ast = 0; aphase ^= 1; }
+                }
             }
             wgmma_wait<0>();
             if (prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev);
+            if (prev_a >= 0 && lane == 0) mbar_arrive(bar_aempty + 8 * prev_a);
             if constexpr (NCAT) {
                 if (!wsplit) {
 #pragma unroll
@@ -467,8 +516,10 @@ int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap&
     p.res_tma = (STG >= 2 && p.tma_out && p.res_split && p_in.res_tma) ? 1 : 0;
     const size_t b_tile = p.bdiag ? (size_t)(BLOCK_N / 16) * 512 : (size_t)BLOCK_N * BLOCK_K * 2;
     size_t stage_bytes = (size_t)p.planes * A_TILE_BYTES + (size_t)p.wplanes * b_tile;
-    if (p.halo) stage_bytes = (((size_t)p.planes * (p.TW + 2) * 128 + 1023) & ~(size_t)1023) + (size_t)p.wplanes * 3 * b_tile;
-    size_t smem = (size_t)STAGES * stage_bytes + (size_t)STG * p.planes * A_TILE_BYTES + 256;
+    const size_t halo_a = ((size_t)p.planes * p.TH * (p.TW + 2) * 128 + 1023) & ~(size_t)1023;
+    if (p.halo) stage_bytes = halo_a + (size_t)p.wplanes * 3 * b_tile;
+    if (p.arow) stage_bytes = (size_t)p.wplanes * b_tile;
+    size_t smem = (size_t)STAGES * stage_bytes + (size_t)STG * p.planes * A_TILE_BYTES + (p.arow ? 2 * halo_a : 0) + 256;
     if (smem > 227 * 1024) return HEAL_ERR_UNSUPPORTED;
     if (p.tma_out && p.res_split && !p.res_tma) return HEAL_ERR_UNSUPPORTED;
     if ((p.blockdiag != 0) != GROUPED || (GROUPED && BLOCK_N != 64)) return HEAL_ERR_UNSUPPORTED;    // the staging epilogue adds a split residual only from TMA loads
@@ -547,7 +598,16 @@ extern "C" int heal_conv2d_tc(const void* in_split, size_t in_plane_stride, int 
     {
         const bool want = env.halo != 0;
         p.bo_mode = env.bo;
-        p.halo = (want && kh == 3 && kw == 3 && stride == 1 && pad == 1 && p.TH == 1 && block_n == 64 && upsample == 1) ? 1 : 0;
+        // Two-row tiles (64-wide maps) only for the grouped convs: their k-block order is the same with or without halo loads
+        // (bit-identical), and with packed diagonal weights their 45 KiB halo stages keep three stages.  A dense halo stage is
+        // 81 KiB (two stages), and no dense 64-wide layer of the product has been measured to gain from that trade.
+        const bool rows_ok = p.TH == 1 || (p.TH == 2 && blockdiag);
+        p.halo = (want && kh == 3 && kw == 3 && stride == 1 && pad == 1 && rows_ok && block_n == 64 && upsample == 1) ? 1 : 0;
+        // 128-wide dense 3x3 (the shrink header): three taps' B tiles do not fit a stage next to an A row, so the A rows get a
+        // ring of their own and each (tap, channel block) k-block brings only its B tile.  Only where it was measured faster:
+        // long K (Cin >= 256) and three weight stages (no split residual, which needs two staging buffers and leaves two).
+        p.arow = (want && kh == 3 && kw == 3 && stride == 1 && pad == 1 && p.TH == 1 && block_n == 128 && !blockdiag && upsample == 1 &&
+                  relu != 2 && Cin >= 256 && !res_split) ? 1 : 0;
     }
     // L2 promotion of the activation / residual loads (HEAL_TC_L2PROMO=256: experiment)
     const CUtensorMapL2promotion act_promo = env.l2promo == 256 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B : CU_TENSOR_MAP_L2_PROMOTION_L2_128B;
@@ -557,7 +617,7 @@ extern "C" int heal_conv2d_tc(const void* in_split, size_t in_plane_stride, int 
         cuuint64_t strides[4] = {(cuuint64_t)in_cstride * 2, (cuuint64_t)W * in_cstride * 2, (cuuint64_t)H * W * in_cstride * 2,
                                  (cuuint64_t)in_plane_stride * 2};
         cuuint32_t box[5] = {(cuuint32_t)BLOCK_K, (cuuint32_t)(p.TW * stride), (cuuint32_t)(p.TH * stride), 1u, (cuuint32_t)planes};
-        if (p.halo) box[1] = (cuuint32_t)(p.TW + 2);
+        if (p.halo || p.arow) box[1] = (cuuint32_t)(p.TW + 2);
         cuuint32_t es[5] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1, 1};
         void* base = (void*)((const __nv_bfloat16*)in_split + in_coffset);
         if (planes == 1) { strides[3] = strides[2] * N; }
