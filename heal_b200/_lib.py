@@ -82,6 +82,12 @@ SIGNATURES = {
     "heal_lss_pool_sorted": (_i, [_vp, _c.c_longlong, _c.c_longlong, _c.c_longlong, _vp, _c.c_longlong, _c.c_longlong, _c.c_longlong,
                                   _vp, _i, _i, _i, _i, _i, _i, _i, _ap, _vp, _sz, _vp]),
     "heal_lss_pool": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
+    "heal_stem_conv_swish": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    "heal_dwconv_bn_swish_workspace": (_sz, [_i, _i, _i, _i]),
+    "heal_dwconv_bn_swish": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "heal_se_gate": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "heal_pwconv": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
+    "heal_upsample2x_concat": (_i, [_ap, _ap, _i, _i, _i, _i, _i, _ap, _i, _vp]),
 }
 
 ERRORS = {-1: "HEAL_ERR_ARG", -2: "HEAL_ERR_WORKSPACE", -3: "HEAL_ERR_LAUNCH", -4: "HEAL_ERR_UNSUPPORTED",

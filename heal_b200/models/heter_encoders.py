@@ -1,5 +1,6 @@
 """Per-modality encoders with the reference's `(data_dict, modality_name) -> (n,C,H,W)` signature
-(opencood/models/heter_encoders.py:22-301).  PointPillar runs PillarVFE + scatter as one kernel."""
+(opencood/models/heter_encoders.py:22-301).  PointPillar runs PillarVFE + scatter as one kernel; Lift-Splat-Shoot builds either of
+the reference's camera encoders (`camera_encoder: EfficientNet` -> CamEncode, `Resnet101` -> CamEncode_Resnet101)."""
 import os as _os
 
 import numpy as np
@@ -195,6 +196,106 @@ class CamEncode_Resnet101(nn.Module):
         return conv_bn_act(y, self._fused_heads(), None, relu=False, out_fmt="f32")
 
 
+class Up(nn.Module):
+    """lss_submodule.py:17-36: bilinear x2 (align_corners=True) of x1, cat([x2, x1_up]), two conv3x3 + BN + ReLU.  `forward_nhwc`
+    writes the concatenation once, in the conv engine's activation format with the channel count rounded up to a multiple of 64
+    (heal_upsample2x_concat), so both convolutions are tensor-core shapes."""
+
+    def __init__(self, in_channels, out_channels, scale_factor=2):
+        super().__init__()
+        self.up = nn.Upsample(scale_factor=scale_factor, mode='bilinear', align_corners=True)
+        self.conv = nn.Sequential(
+            nn.Conv2d(in_channels, out_channels, kernel_size=3, padding=1, bias=False), nn.BatchNorm2d(out_channels), nn.ReLU(inplace=True),
+            nn.Conv2d(out_channels, out_channels, kernel_size=3, padding=1, bias=False), nn.BatchNorm2d(out_channels), nn.ReLU(inplace=True))
+
+    def forward(self, x1, x2):
+        return self.conv(torch.cat([x2, self.up(x1)], dim=1))
+
+    def _first_conv_padded(self):
+        """conv[0] with zero weights for the input channels that pad the concatenation to a multiple of 64."""
+        from ..engine import _sig
+        src = self.conv[0]
+        sig = _sig(src)
+        hit = self.__dict__.get("_conv0_cache")
+        if hit is not None and hit[0] == sig:
+            return hit[1]
+        cin = (src.in_channels + 63) // 64 * 64
+        conv = nn.Conv2d(cin, src.out_channels, 3, padding=1, bias=False).to(src.weight.device)
+        with torch.no_grad():
+            conv.weight.zero_()
+            conv.weight[:, :src.in_channels].copy_(src.weight)
+        self.__dict__["_conv0_cache"] = (sig, conv)                          # not a registered submodule: no state-dict keys
+        return conv
+
+    def forward_nhwc(self, x1, x2):
+        from ..engine import act_fmt, conv_bn_act
+        y = ops.upsample2x_concat(x1, x2, act_fmt())
+        y = conv_bn_act(y, self._first_conv_padded(), self.conv[1], relu=True)
+        return conv_bn_act(y, self.conv[3], self.conv[4], relu=True)
+
+
+class CamEncode(nn.Module):
+    """EfficientNet-B0 trunk + two `Up` stages + depth / image heads (opencood/models/sub_modules/lss_submodule.py:39-138), same
+    attribute names -> same state-dict keys; `trunk` holds efficientnet_pytorch's key names (sub_modules/efficientnet_b0.py).
+    `heads_nhwc` is the GPU path:
+      trunk                     stem, depthwise and pointwise kernels of csrc/mbconv.cu (fp32 channels-last; BN folded; the SE
+                                multiply applied inside the project conv)
+      up1, up2                  heal_upsample2x_concat, then both 3x3 convs + BN + ReLU on the conv engine (wgmma)
+      depth_head | image_head   one fused 1x1 convolution 512 -> D + C, fp32 channels-last output
+    `heads` keeps the plain torch path (CPU-capable; the tests' oracle-side restatement)."""
+
+    def __init__(self, D, C, downsample, ddiscr, mode, use_gt_depth=False, depth_supervision=True):
+        super().__init__()
+        from .sub_modules.efficientnet_b0 import EfficientNetB0
+        self.D, self.C, self.downsample = D, C, downsample
+        self.d_min, self.d_max, self.num_bins = ddiscr[0], ddiscr[1], ddiscr[2]
+        self.mode, self.use_gt_depth, self.depth_supervision = mode, use_gt_depth, depth_supervision
+        if downsample not in (8, 16):
+            raise NotImplementedError(f"img_downsample {downsample}: the EfficientNet encoder produces /8 or /16 feature maps")
+        self.trunk = EfficientNetB0()
+        self.up1 = Up(320 + 112, 512)
+        if downsample == 8:
+            self.up2 = Up(512 + 40, 512)
+        if use_gt_depth:
+            raise NotImplementedError("use_depth_gt is a training-time option outside the inference hot path")
+        self.depth_head = nn.Conv2d(512, self.D, kernel_size=1, padding=0)
+        self.image_head = nn.Conv2d(512, self.C, kernel_size=1, padding=0)
+
+    def _check_sides(self, H, W):
+        """`Up` concatenates the x2-upsampled coarser map with the finer one (lss_submodule.py:108-110); each stride-2 stage maps a
+        side s to s // 2, so the two only agree when no halving that `Up` undoes dropped a row or column."""
+        for name, s in (("height", H), ("width", W)):
+            r = [s]
+            for _ in range(5):
+                r.append(r[-1] // 2)
+            pairs = [(r[5], r[4])] + ([(r[4], r[3])] if self.downsample == 8 else [])
+            for coarse, fine in pairs:
+                if coarse < 1 or 2 * coarse != fine:
+                    raise ValueError(f"image {name} {s}: the EfficientNet feature maps have {name}s {r[3]} (/8), {r[4]} (/16), {r[5]} (/32), "
+                                     f"and {coarse} upsampled x2 does not match {fine}; use image sides that are multiples of 32")
+
+    def heads(self, x):
+        """x (BN, 3|4, H, W) -> (depth_logits (BN,D,fH,fW), feat (BN,C,fH,fW))"""
+        self._check_sides(x.shape[2], x.shape[3])
+        ep = self.trunk.endpoints(x[:, :3])
+        f = self.up1(ep['reduction_5'], ep['reduction_4'])
+        if self.downsample == 8:
+            f = self.up2(f, ep['reduction_3'])
+        return self.depth_head(f), self.image_head(f)
+
+    _fused_heads = CamEncode_Resnet101._fused_heads
+
+    def heads_nhwc(self, x):
+        """x (BN, 3|4, H, W) fp32 CUDA -> Act f32 (BN, H/ds, W/ds, D + C): [depth logits | image features] per pixel."""
+        from ..engine import conv_bn_act
+        self._check_sides(x.shape[2], x.shape[3])
+        r3, r4, r5 = self.trunk.endpoints_nhwc(x.float().contiguous())
+        f = self.up1.forward_nhwc(r5, r4)
+        if self.downsample == 8:
+            f = self.up2.forward_nhwc(f, r3)
+        return conv_bn_act(f, self._fused_heads(), None, relu=False, out_fmt="f32")
+
+
 class LiftSplatShoot(nn.Module):
     """opencood/models/heter_encoders.py:83-241 with the reference's ctor argument and forward signature."""
 
@@ -217,11 +318,12 @@ class LiftSplatShoot(nn.Module):
         self.register_buffer("frustum", self.create_frustum(), persistent=False)
         self.D = self.frustum.shape[0]
         self.camera_encoder_type = args['camera_encoder']
-        if self.camera_encoder_type != 'Resnet101':
-            raise NotImplementedError("camera_encoder 'EfficientNet' needs efficientnet_pytorch + pretrained download; "
-                                      "use 'Resnet101' (SURVEY.md 8c)")
-        self.camencode = CamEncode_Resnet101(self.D, self.camC, self.downsample, self.grid_conf['ddiscr'],
-                                             self.grid_conf['mode'], args['use_depth_gt'], args['depth_supervision'])
+        encoders = {'EfficientNet': CamEncode, 'Resnet101': CamEncode_Resnet101}
+        if self.camera_encoder_type not in encoders:
+            raise NotImplementedError(f"camera_encoder '{self.camera_encoder_type}': the reference builds 'EfficientNet' or 'Resnet101' "
+                                      "(opencood/models/heter_encoders.py:103-108)")
+        self.camencode = encoders[self.camera_encoder_type](self.D, self.camC, self.downsample, self.grid_conf['ddiscr'],
+                                                            self.grid_conf['mode'], args['use_depth_gt'], args['depth_supervision'])
         if self._nx_host[2] != 1:
             raise NotImplementedError("heal_lss_pool supports a single z slice (every HEAL yaml uses zbound with nz == 1)")
 

@@ -974,6 +974,131 @@ def lss_pool_sorted(logits: torch.Tensor, l_strides, feat: torch.Tensor, f_strid
 
 
 # ------------------------------------------------------------------------------------------------
+# EfficientNet-B0 camera trunk (csrc/mbconv.cu): dense channels-last fp32 tensors, BN folded on the host in fp64
+# ------------------------------------------------------------------------------------------------
+def _fold_conv_bn(conv, bn):
+    """(weight * bn scale (Cout, Cin/g, kh, kw), bias) in fp64 on the host."""
+    w = conv.weight.detach().double().cpu()
+    scale, shift = _bn_scale_shift(bn, w.shape[0])
+    b = shift + (conv.bias.detach().double().cpu() * scale if conv.bias is not None else 0)
+    return w * scale[:, None, None, None], b
+
+
+def pack_stem_conv(conv, bn):
+    """Conv2d(3, 32, 3, stride 2) + BN -> (weight (27, 32), row = (ci*3 + ky)*3 + kx; bias (32)) for heal_stem_conv_swish."""
+    w, b = _fold_conv_bn(conv, bn)
+    assert w.shape == (32, 3, 3, 3) and conv.stride == (2, 2)
+    return w.reshape(32, 27).t().contiguous().float(), b.float().contiguous()
+
+
+def pack_dwconv(conv, bn):
+    """depthwise Conv2d(C, C, k, groups=C) + BN -> (weight (k*k, C) tap-major, bias (C)) for heal_dwconv_bn_swish."""
+    w, b = _fold_conv_bn(conv, bn)
+    C, one, k, k2 = w.shape
+    assert one == 1 and k == k2 and conv.groups == C
+    return w.reshape(C, k * k).t().contiguous().float(), b.float().contiguous()
+
+
+def pack_pwconv(conv, bn):
+    """Conv2d(Cin, Cout, 1) (+ BN) -> (weight (Cin, Cout), bias (Cout)) for heal_pwconv."""
+    w, b = _fold_conv_bn(conv, bn)
+    assert w.shape[2:] == (1, 1) and conv.groups == 1
+    return w[:, :, 0, 0].t().contiguous().float(), b.float().contiguous()
+
+
+def pack_se(se_reduce, se_expand):
+    """The two biased 1x1 convs of squeeze-and-excitation -> (w_reduce (Csq, C), b_reduce, w_expand_t (Csq, C), b_expand)."""
+    wr, we = se_reduce.weight.detach()[:, :, 0, 0], se_expand.weight.detach()[:, :, 0, 0]
+    return (wr.float().contiguous().cpu(), se_reduce.bias.detach().float().contiguous().cpu(),
+            we.t().float().contiguous().cpu(), se_expand.bias.detach().float().contiguous().cpu())
+
+
+def _dense_f32(a: Act):
+    assert a.fmt == "f32" and a.cstride == a.C and a.t.is_contiguous(), "the MBConv kernels read dense fp32 channels-last maps"
+
+
+@_guard
+def stem_conv_swish(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor) -> Act:
+    """x (N, 3|4, H, W) fp32 NCHW -> Act f32 (N, (H-2)//2+1, (W-2)//2+1, 32): 3x3/2 conv of the first 3 channels, pad (0, 1), swish."""
+    _need_cuda(x, weight, bias)
+    assert x.dtype == torch.float32 and x.dim() == 4 and x.is_contiguous() and weight.shape == (27, 32)
+    N, Cx, H, W = x.shape
+    Ho, Wo = (H - 2) // 2 + 1, (W - 2) // 2 + 1
+    out = act_empty(N, Ho, Wo, 32, "f32", x.device)
+    with _Prof("stem_conv_swish", 2.0 * N * Ho * Wo * 32 * 27, 4.0 * N * (3 * H * W + Ho * Wo * 32)):
+        _call("heal_stem_conv_swish", _p(x), N, Cx, H, W, _p(weight), _p(bias), _p(out.t))
+    return out
+
+
+@_guard
+def dwconv_bn_swish(x: Act, weight: torch.Tensor, bias: torch.Tensor, ksize: int, stride: int, pads):
+    """Depthwise conv + folded BN + swish.  pads = (top, bottom, left, right).  Returns (Act f32, sums (N, C) fp32): sums is the sum
+    of the output over its pixels (the squeeze of squeeze-and-excitation before the division), bit-identical run to run."""
+    _need_cuda(weight, bias)
+    _dense_f32(x)
+    N, H, W, C = x.N, x.H, x.W, x.C
+    assert weight.shape == (ksize * ksize, C)
+    pt, pb, pl, pr = pads
+    Ho, Wo = (H + pt + pb - ksize) // stride + 1, (W + pl + pr - ksize) // stride + 1
+    out = act_empty(N, Ho, Wo, C, "f32", x.device)
+    sums = torch.empty((N, C), dtype=torch.float32, device=x.device)
+    ws = _workspace(x.device, lib.heal_dwconv_bn_swish_workspace(N, C, Ho, Wo))
+    with _Prof("dwconv_bn_swish", 2.0 * N * Ho * Wo * C * ksize * ksize, 4.0 * N * C * (H * W + Ho * Wo)):
+        _call("heal_dwconv_bn_swish", _p(x.t), N, H, W, C, _p(weight), _p(bias), int(ksize), int(stride), int(pt), int(pl),
+              Ho, Wo, _p(out.t), _p(sums), _p(ws), ws.numel())
+    return out, sums
+
+
+@_guard
+def se_gate(sums: torch.Tensor, hw: int, w_reduce, b_reduce, w_expand_t, b_expand) -> torch.Tensor:
+    """sums (N, C) over hw pixels -> gate (N, C) = sigmoid(expand(swish(reduce(sums / hw))))."""
+    _need_cuda(sums, w_reduce, b_reduce, w_expand_t, b_expand)
+    N, C = sums.shape
+    Csq = w_reduce.shape[0]
+    assert sums.is_contiguous() and w_reduce.shape == (Csq, C) and w_expand_t.shape == (Csq, C)
+    gate = torch.empty_like(sums)
+    with _Prof("se_gate", 4.0 * N * C * Csq, 8.0 * C * Csq + 8.0 * N * C):
+        _call("heal_se_gate", _p(sums), N, C, Csq, int(hw), _p(w_reduce), _p(b_reduce), _p(w_expand_t), _p(b_expand), _p(gate))
+    return gate
+
+
+@_guard
+def pwconv(x: Act, weight: torch.Tensor, bias: torch.Tensor, gate: Optional[torch.Tensor] = None, swish: bool = False,
+           residual: Optional[Act] = None) -> Act:
+    """1x1 conv with folded BN: out = act((x * gate[image]) @ weight + bias) + residual.  weight (Cin, Cout)."""
+    _need_cuda(weight, bias, gate)
+    _dense_f32(x)
+    N, H, W, Cin = x.N, x.H, x.W, x.C
+    Cout = weight.shape[1]
+    assert weight.shape[0] == Cin and weight.is_contiguous()
+    if gate is not None:
+        assert gate.shape == (N, Cin) and gate.is_contiguous()
+    if residual is not None:
+        _dense_f32(residual)
+        assert (residual.N, residual.H, residual.W, residual.C) == (N, H, W, Cout)
+    out = act_empty(N, H, W, Cout, "f32", x.device)
+    with _Prof("pwconv", 2.0 * N * H * W * Cin * Cout,
+               4.0 * N * H * W * (Cin + Cout * (2 if residual is not None else 1)) + 4.0 * Cin * Cout):
+        _call("heal_pwconv", _p(x.t), N, H * W, Cin, Cout, _p(weight), _p(bias), _p(gate), 1 if swish else 0,
+              _p(residual.t) if residual is not None else _vp(0), _p(out.t))
+    return out
+
+
+@_guard
+def upsample2x_concat(x1: Act, x2: Act, out_fmt: str) -> Act:
+    """`Up`'s front half (lss_submodule.py:33-35): Act (N, 2*H1, 2*W1, C) in `out_fmt` holding [x2 | bilinear x2 (align_corners=True) of
+    x1 | zeros], C = C2 + C1 rounded up to a multiple of 64 (the tensor-core convolution's input-channel granularity)."""
+    N, H1, W1 = x1.N, x1.H, x1.W
+    assert (x2.N, x2.H, x2.W) == (N, 2 * H1, 2 * W1)
+    C = (x1.C + x2.C + 63) // 64 * 64
+    out = act_empty(N, 2 * H1, 2 * W1, C, out_fmt, x1.device)
+    with _Prof("upsample2x_concat", 8.0 * N * 4 * H1 * W1 * x1.C,
+               N * H1 * W1 * (x1.C * BPE[x1.fmt] + 4.0 * x2.C * BPE[x2.fmt] + 4.0 * C * BPE[out_fmt])):
+        _call("heal_upsample2x_concat", x1.view(), x2.view(), N, H1, W1, x1.C, x2.C, out.view(), C)
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
 # sparse 3-D convolution (SECOND)
 # ------------------------------------------------------------------------------------------------
 class SparseTensor:

@@ -408,6 +408,36 @@ int heal_dwconv_layernorm(const heal_act_t* in, int N, int H, int W, int C, cons
  * (N,H/2,W/2,4C) with channel block (y&1)*2+(x&1) -- the phase-major output of the space-to-depth form of the 7x7/2 stem conv. */
 int heal_maxpool3x3s2(const heal_act_t* in, int N, int H, int W, int C, int depth_to_space_in, const heal_act_t* out, void* stream);
 
+/* ---- EfficientNet-B0 camera trunk of Lift-Splat-Shoot (`camera_encoder: EfficientNet`, SURVEY.md 8c) ---------------------
+ * opencood/models/sub_modules/lss_submodule.py:87-111 runs efficientnet_pytorch's stem and MBConv blocks, then `Up` (:17-36).
+ * Trunk tensors are dense channels-last fp32 (N,H,W,C); BatchNorm (eps 1e-3) is folded into weight / bias by the caller;
+ * swish(x) = x * sigmoid(x).  Channel counts are multiples of 4.
+ *
+ * heal_stem_conv_swish: 3x3 / stride 2 conv 3 -> 32 reading the first 3 of `image_channels` planes of the NCHW image, zero pad
+ *   0 before and 1 after in y and x (the package's static "same" padding), + bias, swish.  weight [27][32], row (ci*3+ky)*3+kx.
+ *   out (N, (H-2)/2+1, (W-2)/2+1, 32).
+ * heal_dwconv_bn_swish: depthwise ksize in {3,5}, stride in {1,2}, `pad_top` / `pad_left` zeros before the image (what lies after
+ *   follows from Ho, Wo), + bias, swish.  weight [ksize*ksize][C] tap-major.  Also writes sums (N,C) = the sum of `out` over its
+ *   pixels, added in a fixed order (bit-identical run to run).  workspace >= heal_dwconv_bn_swish_workspace(N, C, Ho, Wo).
+ * heal_se_gate: gate (N,C) = sigmoid(W_e swish(W_r (sums / HW) + b_r) + b_e).  w_reduce [Csq][C], w_expand_t [Csq][C]
+ *   (the expand weight transposed); C <= 1152, Csq <= 64.
+ * heal_pwconv: 1x1 conv out = act(sum_ci in[.., ci] * gate[n, ci] * weight[ci][co] + bias[co]) + residual.  weight [Cin][Cout];
+ *   gate (N,Cin) or NULL; swish_epilogue 0 | 1; residual (N,HW,Cout) or NULL.
+ * heal_upsample2x_concat: out (N, 2*H1, 2*W1, Cout) = [x2 (C2 channels) | bilinear x2, align_corners=True, of x1 (C1 channels) |
+ *   zeros]; any storage format on each side (the zero tail pads the channel count for the tensor-core convolution that follows). */
+int heal_stem_conv_swish(const float* image, int N, int image_channels, int H, int W, const float* weight, const float* bias,
+                         float* out, void* stream);
+size_t heal_dwconv_bn_swish_workspace(int N, int C, int Ho, int Wo);
+int heal_dwconv_bn_swish(const float* in, int N, int H, int W, int C, const float* weight, const float* bias, int ksize,
+                         int stride, int pad_top, int pad_left, int Ho, int Wo, float* out, float* sums,
+                         void* workspace, size_t workspace_bytes, void* stream);
+int heal_se_gate(const float* sums, int N, int C, int Csq, int HW, const float* w_reduce, const float* b_reduce,
+                 const float* w_expand_t, const float* b_expand, float* gate, void* stream);
+int heal_pwconv(const float* in, int N, int HW, int Cin, int Cout, const float* weight, const float* bias, const float* gate,
+                int swish_epilogue, const float* residual, float* out, void* stream);
+int heal_upsample2x_concat(const heal_act_t* x1, const heal_act_t* x2, int N, int H1, int W1, int C1, int C2,
+                           const heal_act_t* out, int Cout, void* stream);
+
 /* ---- peer-to-peer exchange over NVLink / NVSwitch (agent-per-GPU partition, SURVEY.md 8e) ---------------------
  * The buffers are SYMMETRIC: every rank allocated the same size and mapped every peer's copy (peer_*_host[r] = this process's
  * device pointer to rank r's copy; [self] = the local one).
