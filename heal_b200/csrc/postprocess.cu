@@ -5,7 +5,7 @@
 //            :840-890 (remove_large_pred_bbx / remove_bbx_abnormal_z), :384-421 (mask_boxes_outside_range_numpy);
 //            opencood/utils/common_utils.py:104-113 (limit_period), :230-270 (compute_iou / convert_format).
 // Pipeline (all on the caller's stream, no host sync; the counts stay on the device):
-//   k_decode      one thread per anchor: sigmoid, score threshold, delta decode, direction-bin fix, 8 corners, ego projection,
+//   k_decode      one thread per anchor (late entry point: blockIdx.y = cav, its 4x4 transform read on the device): sigmoid, score threshold, delta decode, direction-bin fix, 8 corners, ego projection,
 //                 size / z filters -> sort key (score or -1) + the 24 corner floats
 //   cub radix sort (descending, stable) of (key, anchor index): the reference's `scores.argsort()[::-1][:top]`
 //   k_gather_top  the `top` best: corners, score, the 2-D polygon (corners 0..3, x/y) made counter-clockwise, its area (fp64)
@@ -28,7 +28,8 @@ struct DecP {
     const float* anchors;          // (H,W,A,7)
     int H, W, A, bins, hwl;
     float thr, dir_offset;
-    float T[12];                   // rows 0..2 of the 4x4 cav -> ego transform
+    float T[12];                   // rows 0..2 of the 4x4 cav -> ego transform (host-given; used when Tdev is null)
+    const float* Tdev;             // or: device (gridDim.y, 4, 4) row-major transforms, cav = blockIdx.y, heads (gridDim.y, H, W, .)
     float* keys; int* vals; float* cand;    // per anchor: sort key, index, 24 corner floats
     int* counters;                 // [0] above the score threshold, [1] after the size / z filters
 };
@@ -42,8 +43,12 @@ k_decode(DecP p) {
     const int n = p.H * p.W * p.A;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const int a = i % p.A; const size_t pix = (size_t)(i / p.A);
-    const int slot = p.base + i;
+    const int cav = blockIdx.y;
+    const int a = i % p.A; const size_t pix = (size_t)cav * p.H * p.W + (size_t)(i / p.A);
+    const int slot = p.base + cav * n + i;
+    float T[12];
+#pragma unroll
+    for (int k = 0; k < 12; ++k) T[k] = p.Tdev ? __ldg(p.Tdev + (size_t)cav * 16 + k) : p.T[k];
     p.vals[slot] = slot;
     float key = -1.f;
     const float prob = 1.f / (1.f + expf(-ldf(p.cls, pix, a)));
@@ -82,9 +87,9 @@ k_decode(DecP p) {
         for (int k = 0; k < 8; ++k) {
             const float lx = dx * (sx[k] * 0.5f), ly = dy * (sy[k] * 0.5f), lz = dz * (sz[k] * 0.5f);
             const float x = lx * ca + ly * (-sa) + b[0], y = lx * sa + ly * ca + b[1], z = lz + b[2];
-            const float X = p.T[0] * x + p.T[1] * y + p.T[2] * z + p.T[3];
-            const float Y = p.T[4] * x + p.T[5] * y + p.T[6] * z + p.T[7];
-            const float Z = p.T[8] * x + p.T[9] * y + p.T[10] * z + p.T[11];
+            const float X = T[0] * x + T[1] * y + T[2] * z + T[3];
+            const float Y = T[4] * x + T[5] * y + T[6] * z + T[7];
+            const float Z = T[8] * x + T[9] * y + T[10] * z + T[11];
             c[3 * k] = X; c[3 * k + 1] = Y; c[3 * k + 2] = Z;
             xmin = fminf(xmin, X); xmax = fmaxf(xmax, X); ymin = fminf(ymin, Y); ymax = fmaxf(ymax, Y);
             zmin = fminf(zmin, Z); zmax = fmaxf(zmax, Z);
@@ -286,6 +291,31 @@ WsLayout layout(int n, int top) {
     return L;
 }
 
+// The chain after the decode, shared by the multi and the late entry points: sort -> k_gather_top -> k_iou_mask -> k_nms_finish
+// -> k_emit (+ the stats copy).  `p` holds the workspace pointers the decode filled.
+int sort_nms_emit(const WsLayout& L, uint8_t* ws, const DecP& p, int n, int top, const float* range6_host, float nms_threshold,
+                  float* boxes_out, float* scores_out, int* count_out, int* stats_out, cudaStream_t st) {
+    size_t cb = L.cub_bytes;
+    if (cub::DeviceRadixSort::SortPairsDescending(ws + L.cub, cb, (const float*)p.keys, (float*)(ws + L.keys_out), (const int*)p.vals,
+                                                  (int*)(ws + L.vals_out), n, 0, 32, st) != cudaSuccess) return HEAL_ERR_LAUNCH;
+    const float* r = range6_host;
+    const float rl[6] = {r ? r[0] : 0.f, r ? r[1] : 0.f, r ? r[2] : 0.f, r ? r[3] : 0.f, r ? r[4] : 0.f, r ? r[5] : 0.f};
+    k_gather_top<<<(top + 127) / 128, 128, 0, st>>>((const float*)(ws + L.keys_out), (const int*)(ws + L.vals_out), p.cand, p.counters, top,
+                                                    (float*)(ws + L.top_c), (float*)(ws + L.top_s), (double*)(ws + L.poly),
+                                                    rl[0], rl[1], rl[2], rl[3], rl[4], rl[5], r ? 1 : 0, (unsigned char*)(ws + L.inrange));
+    dim3 g((top + 63) / 64, (top + 63) / 64);
+    k_iou_mask<<<g, 64, 0, st>>>((const double*)(ws + L.poly), p.counters, top, nms_threshold, L.words, (unsigned long long*)(ws + L.mask));
+    const size_t nms_smem = (size_t)top * L.words * 8 + (((size_t)top + 15) & ~(size_t)15);
+    static size_t nms_attr[HEAL_MAX_DEVICES] = {};
+    if (!heal_ensure_dyn_smem(k_nms_finish, nms_smem, nms_attr)) return HEAL_ERR_LAUNCH;
+    k_nms_finish<<<1, 1024, nms_smem, st>>>((const unsigned long long*)(ws + L.mask), (const unsigned char*)(ws + L.inrange), p.counters, top,
+                                            L.words, (int*)(ws + L.keep), count_out);
+    k_emit<<<top, 32, 0, st>>>((const int*)(ws + L.keep), count_out, (const float*)(ws + L.top_c), (const float*)(ws + L.top_s),
+                               boxes_out, scores_out);
+    if (stats_out) cudaMemcpyAsync(stats_out, p.counters, 8, cudaMemcpyDeviceToDevice, st);
+    return HEAL_OK;
+}
+
 }  // namespace
 
 extern "C" size_t heal_postprocess_workspace(int H, int W, int anchors_per_cell, int top) {
@@ -312,6 +342,7 @@ extern "C" int heal_box_decode_nms_multi(const heal_cav_heads_t* cavs_host, int 
     p.thr = score_threshold; p.dir_offset = dir_offset;
     p.keys = (float*)(ws + L.keys_in); p.vals = (int*)(ws + L.vals_in); p.cand = (float*)(ws + L.cand);
     p.counters = (int*)(ws + L.counters);
+    p.Tdev = nullptr;
     cudaMemsetAsync(p.counters, 0, 16, st);
     cudaMemsetAsync(ws + L.mask, 0, (size_t)top * L.words * 8, st);
     for (int c = 0; c < n_cav; ++c) {
@@ -326,25 +357,43 @@ extern "C" int heal_box_decode_nms_multi(const heal_cav_heads_t* cavs_host, int 
         for (int k = 0; k < 12; ++k) p.T[k] = h.transform4x4_host[k];
         k_decode<<<(n1 + 255) / 256, 256, 0, st>>>(p);
     }
-    size_t cb = L.cub_bytes;
-    if (cub::DeviceRadixSort::SortPairsDescending(ws + L.cub, cb, (const float*)p.keys, (float*)(ws + L.keys_out), (const int*)p.vals,
-                                                  (int*)(ws + L.vals_out), n, 0, 32, st) != cudaSuccess) return HEAL_ERR_LAUNCH;
-    const float* r = range6_host;
-    const float rl[6] = {r ? r[0] : 0.f, r ? r[1] : 0.f, r ? r[2] : 0.f, r ? r[3] : 0.f, r ? r[4] : 0.f, r ? r[5] : 0.f};
-    k_gather_top<<<(top + 127) / 128, 128, 0, st>>>((const float*)(ws + L.keys_out), (const int*)(ws + L.vals_out), p.cand, p.counters, top,
-                                                    (float*)(ws + L.top_c), (float*)(ws + L.top_s), (double*)(ws + L.poly),
-                                                    rl[0], rl[1], rl[2], rl[3], rl[4], rl[5], r ? 1 : 0, (unsigned char*)(ws + L.inrange));
-    dim3 g((top + 63) / 64, (top + 63) / 64);
-    k_iou_mask<<<g, 64, 0, st>>>((const double*)(ws + L.poly), p.counters, top, nms_threshold, L.words, (unsigned long long*)(ws + L.mask));
-    const size_t nms_smem = (size_t)top * L.words * 8 + (((size_t)top + 15) & ~(size_t)15);
-    static size_t nms_attr[HEAL_MAX_DEVICES] = {};
-    if (!heal_ensure_dyn_smem(k_nms_finish, nms_smem, nms_attr)) return HEAL_ERR_LAUNCH;
-    k_nms_finish<<<1, 1024, nms_smem, st>>>((const unsigned long long*)(ws + L.mask), (const unsigned char*)(ws + L.inrange), p.counters, top,
-                                            L.words, (int*)(ws + L.keep), count_out);
-    k_emit<<<top, 32, 0, st>>>((const int*)(ws + L.keep), count_out, (const float*)(ws + L.top_c), (const float*)(ws + L.top_s),
-                               boxes_out, scores_out);
-    if (stats_out) cudaMemcpyAsync(stats_out, p.counters, 8, cudaMemcpyDeviceToDevice, st);
+    const int rc = sort_nms_emit(L, ws, p, n, top, range6_host, nms_threshold, boxes_out, scores_out, count_out, stats_out, st);
+    if (rc != HEAL_OK) return rc;
     return heal_check_launch(4 + n_cav);
+}
+
+extern "C" int heal_box_decode_nms_late(const heal_act_t* cls, const heal_act_t* reg, const heal_act_t* dir, const float* anchors,
+                                        const float* transforms_dev, int n_cav, int H, int W, int anchors_per_cell,
+                                        float score_threshold, float dir_offset, int num_bins, int order_hwl, float nms_threshold,
+                                        int top, const float* range6_host, float* boxes_out, float* scores_out, int* count_out,
+                                        int* stats_out, void* workspace, size_t workspace_bytes, void* stream_) {
+    if (n_cav < 1 || n_cav > 16 || !cls || !cls->data || !reg || !reg->data || !anchors || !transforms_dev) return HEAL_ERR_ARG;
+    if (!boxes_out || !scores_out || !count_out || !workspace) return HEAL_ERR_ARG;
+    if (H < 1 || W < 1 || anchors_per_cell < 1 || top < 1 || top > 1320 || num_bins < 1) return HEAL_ERR_ARG;
+    if (cls->fmt != 0 || reg->fmt != 0 || (dir && dir->data && dir->fmt != 0)) return HEAL_ERR_UNSUPPORTED;
+    const int n1 = H * W * anchors_per_cell;
+    const long long nt = (long long)n1 * n_cav;
+    if (nt >= (1LL << 30)) return HEAL_ERR_UNSUPPORTED;
+    const int n = (int)nt;
+    const WsLayout L = layout(n, top);
+    if (workspace_bytes < L.total) return HEAL_ERR_ARG;
+    cudaStream_t st = (cudaStream_t)stream_;
+    uint8_t* ws = (uint8_t*)workspace;
+    DecP p;
+    p.H = H; p.W = W; p.A = anchors_per_cell; p.bins = num_bins; p.hwl = order_hwl ? 1 : 0;
+    p.thr = score_threshold; p.dir_offset = dir_offset;
+    p.keys = (float*)(ws + L.keys_in); p.vals = (int*)(ws + L.vals_in); p.cand = (float*)(ws + L.cand);
+    p.counters = (int*)(ws + L.counters);
+    p.cls = to_view(cls); p.reg = to_view(reg);
+    if (dir && dir->data) p.dir = to_view(dir); else { p.dir = p.cls; p.dir.p = nullptr; }
+    p.iou = p.cls; p.iou.p = nullptr;
+    p.anchors = anchors; p.base = 0; p.Tdev = transforms_dev;
+    cudaMemsetAsync(p.counters, 0, 16, st);
+    cudaMemsetAsync(ws + L.mask, 0, (size_t)top * L.words * 8, st);
+    k_decode<<<dim3((n1 + 255) / 256, n_cav), 256, 0, st>>>(p);
+    const int rc = sort_nms_emit(L, ws, p, n, top, range6_host, nms_threshold, boxes_out, scores_out, count_out, stats_out, st);
+    if (rc != HEAL_OK) return rc;
+    return heal_check_launch(5);
 }
 
 extern "C" int heal_box_decode_nms(const heal_act_t* cls, const heal_act_t* reg, const heal_act_t* dir, const float* anchors,

@@ -225,3 +225,103 @@ class FramePipeline:
                 s.wait_stream(cur)
             else:
                 cur.wait_stream(s)
+
+
+class LateFusionGraph:
+    """Late fusion of one scene as ONE captured graph: a single-agent model's `grouped_heads` (one batched forward per modality,
+    every cav's heads in one (n_cav, H, W, S) buffer) and heal_box_decode_nms_late (decode with the transforms read on the device,
+    sort, rotated NMS, range mask).  The reference runs one model call per cav, then the post-processor on the host.
+
+        g = LateFusionGraph(model, ["m1", "m1", "m2"], {"m1": 200000, "m2": (4, 256, 704)}, hypes["postprocess"])
+        g.load(batch_data)            # {cav_id: {inputs_<m>: ..., transformation_matrix: 4x4}} in the captured modality order
+        out = g.replay()              # out.boxes[:out.count], out.scores[:out.count] on the device, no host sync
+
+    `capacities[m]`: for a lidar modality the point capacity of ALL its cavs together (raw clouds, `points` + `agent_offsets`; the
+    live counts travel in the offsets), for a camera modality (cameras, image height, image width) per cav.  The poses are
+    inputs: replaying the graph for another scene uses that scene's transforms."""
+
+    CAMERA_KEYS = ("rots", "trans", "intrins", "post_rots", "post_trans")
+
+    def __init__(self, model, modality_of_each_cav, capacities, postprocess_params, device=None, warmup: int = 2, top: int = 1000):
+        from . import ops
+        from .data_utils.post_processor.voxel_postprocessor import VoxelPostprocessor
+        dev = device or next(model.parameters()).device
+        self.modalities = list(modality_of_each_cav)
+        n = len(self.modalities)
+        self.groups = {}
+        for i, m in enumerate(self.modalities):
+            self.groups.setdefault(m, []).append(i)
+        self.inputs = {}
+        for m, idx in self.groups.items():
+            k = len(idx)
+            if model.sensor_type_dict[m] == "camera":
+                cams, h, w = capacities[m]
+                self.inputs[m] = {"imgs": torch.zeros((k, cams, 3, h, w), dtype=torch.float32, device=dev),
+                                  "rots": torch.eye(3, device=dev).repeat(k, cams, 1, 1),
+                                  "trans": torch.zeros((k, cams, 3), dtype=torch.float32, device=dev),
+                                  "intrins": torch.eye(3, device=dev).repeat(k, cams, 1, 1),
+                                  "post_rots": torch.eye(3, device=dev).repeat(k, cams, 1, 1),
+                                  "post_trans": torch.zeros((k, cams, 3), dtype=torch.float32, device=dev)}
+            else:
+                self.inputs[m] = {"points": torch.zeros((int(capacities[m]), 4), dtype=torch.float32, device=dev),
+                                  "agent_offsets": torch.zeros((k + 1,), dtype=torch.int32, device=dev)}
+        self.transforms = torch.eye(4, dtype=torch.float32, device=dev).repeat(n, 1, 1).contiguous()
+        pp = VoxelPostprocessor(postprocess_params, False)
+        self.anchors = torch.from_numpy(pp.generate_anchor_box()).to(device=dev, dtype=torch.float32).contiguous()
+        A = self.anchors.shape[2]
+        dargs = postprocess_params.get('dir_args', {})
+        bins = int(dargs.get('num_bins', 2))
+        self.buffers = ops.PostprocessBuffers(self.anchors.shape[0] * n, self.anchors.shape[1], A, top, dev)
+
+        def run():
+            y, _ = model.grouped_heads(self.groups, self.inputs, n)
+            return ops.box_decode_nms_late(y, y, y, self.anchors, self.transforms,
+                                           postprocess_params['target_args']['score_threshold'], postprocess_params['nms_thresh'],
+                                           dir_offset=dargs.get('dir_offset', 0.0), num_bins=bins, order=postprocess_params['order'],
+                                           gt_range=postprocess_params['gt_range'], top=top, buffers=self.buffers,
+                                           coffsets=(0, A, 8 * A))
+
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side), torch.no_grad():
+            for _ in range(warmup):
+                run()
+        torch.cuda.current_stream(dev).wait_stream(side)
+        torch.cuda.synchronize(dev)
+        self.graph = torch.cuda.CUDAGraph()
+        l0 = lib.heal_launch_count()
+        with torch.no_grad(), torch.cuda.graph(self.graph, capture_error_mode="thread_local"):
+            self.out = run()
+        self.kernels_per_replay = int(lib.heal_launch_count() - l0)
+
+    def load(self, batch_data):
+        """Copy a scene's inputs and cav -> ego transforms into the captured buffers (asynchronous copies on the current stream).
+        The cavs must come in the captured modality order; each lidar cav carries one raw cloud (`points`, `agent_offsets`)."""
+        from .models.heter_model_late import modality_of
+        cavs = list(batch_data.keys())
+        mods = [modality_of(batch_data[c]) for c in cavs]
+        if mods != self.modalities:
+            raise ValueError(f"scene modalities {mods}, the graph was captured for {self.modalities}")
+        for m, idx in self.groups.items():
+            buf = self.inputs[m]
+            if "points" in buf:
+                offs, total = [0], 0
+                for j, i in enumerate(idx):
+                    pts = batch_data[cavs[i]][f"inputs_{m}"]["points"]
+                    if total + pts.shape[0] > buf["points"].shape[0]:
+                        raise ValueError(f"{m}: the scene has more points than the graph's capacity {buf['points'].shape[0]}")
+                    buf["points"][total:total + pts.shape[0]].copy_(pts, non_blocking=True)
+                    total += pts.shape[0]
+                    offs.append(total)
+                buf["agent_offsets"].copy_(torch.tensor(offs, dtype=torch.int32), non_blocking=True)
+            else:
+                for j, i in enumerate(idx):
+                    src = batch_data[cavs[i]][f"inputs_{m}"]
+                    for k in ("imgs",) + self.CAMERA_KEYS:
+                        buf[k][j].copy_(src[k][0][:, :3] if k == "imgs" else src[k][0], non_blocking=True)
+        T = torch.stack([torch.as_tensor(batch_data[c]['transformation_matrix']).reshape(4, 4).to(torch.float32) for c in cavs])
+        self.transforms.copy_(T, non_blocking=True)
+
+    def replay(self):
+        self.graph.replay()
+        return self.out

@@ -8,6 +8,8 @@ _MAP = {
     "opencood.models.heter_pyramid_collab": "heal_b200.models.heter_pyramid_collab",
     "opencood.models.heter_model_baseline": "heal_b200.models.heter_model_baseline",
     "opencood.models.heter_model_baseline_ms": "heal_b200.models.heter_model_baseline_ms",
+    "opencood.models.heter_model_late": "heal_b200.models.heter_model_late",
+    "opencood.models.heter_pyramid_single": "heal_b200.models.heter_pyramid_single",
     "opencood.models.point_pillar": "heal_b200.models.point_pillar",
     "opencood.models.heter_encoders": "heal_b200.models.heter_encoders",
     "opencood.models.fuse_modules.pyramid_fuse": "heal_b200.models.fuse_modules.pyramid_fuse",
@@ -25,8 +27,9 @@ _MAP = {
 
 def install_gpu_postprocessor():
     """Opt-in: make the reference's post-processor registry (opencood/data_utils/post_processor/__init__.py `__all__`) hand out a
-    SUBCLASS of its own VoxelPostprocessor whose `post_process` runs on the GPU for early / intermediate fusion and falls back to
-    the reference implementation for everything else (late fusion, iou_preds, CPU tensors).  All label / collate / gt-box methods
+    SUBCLASS of its own VoxelPostprocessor whose `post_process` runs on the GPU for early, intermediate and late fusion (one cav or
+    up to 16 cavs with one head geometry, with or without iou_preds) and falls back to the reference implementation for everything
+    else (CPU tensors, anchor-free heads, cavs whose head maps differ in size).  All label / collate / gt-box methods
     the datasets call are inherited unchanged."""
     from .data_utils.post_processor.voxel_postprocessor import make_reference_subclass
     reg = importlib.import_module("opencood.data_utils.post_processor")

@@ -36,14 +36,21 @@ class FusedHeads:
                 conv.bias.copy_(torch.cat([h.bias for h in self.heads], 0))
             self._conv, self._sig = conv, sig
 
-    def __call__(self, x_nhwc):
+    def act(self, x_nhwc, out=None):
+        """The fused (B,H,W,sum) fp32 output as an Act; `out` may be an f32 Act of that shape (e.g. images of a larger buffer)."""
         self.prepare()
-        y = conv_bn_act(x_nhwc, self._conv, None, relu=False, out_fmt="f32").t          # (B,H,W,sum) fp32
+        return conv_bn_act(x_nhwc, self._conv, None, relu=False, out=out, out_fmt="f32")
+
+    def split(self, y):
+        """(B,H,W,sum) fp32 -> one logical-NCHW tensor per head."""
         outs, o = [], 0
         for h in self.heads:
             outs.append(y[..., o:o + h.out_channels].permute(0, 3, 1, 2).contiguous())
             o += h.out_channels
         return outs
+
+    def __call__(self, x_nhwc):
+        return self.split(self.act(x_nhwc).t)
 
 
 class HeterPyramidCollab(nn.Module):

@@ -1464,3 +1464,58 @@ def box_decode_nms_multi(cavs, score_threshold: float, nms_threshold: float, dir
               _p(buffers.boxes), _p(buffers.scores), _p(buffers.count), _p(buffers.stats),
               _p(buffers.workspace), buffers.workspace.numel())
     return buffers
+
+
+def _late_heads(t, name: str) -> Act:
+    """box_decode_nms_late's head argument: an f32 Act, or a logical (n, C, H, W) fp32 CUDA tensor."""
+    if isinstance(t, Act):
+        if t.fmt != "f32":
+            raise ValueError(f"{name}: the late decode reads fp32 heads, got an Act in '{t.fmt}'")
+        return t
+    if not isinstance(t, torch.Tensor) or t.dim() != 4 or t.dtype != torch.float32:
+        raise ValueError(f"{name}: expected a (n_cav, C, H, W) fp32 tensor or an f32 Act")
+    return to_act(t)
+
+
+@_guard
+def box_decode_nms_late(cls_preds, reg_preds, dir_preds, anchors: torch.Tensor, transforms: torch.Tensor, score_threshold: float,
+                        nms_threshold: float, dir_offset: float = 0.0, num_bins: int = 2, order: str = "hwl", gt_range=None,
+                        top: int = 1000, buffers: Optional[PostprocessBuffers] = None, coffsets=(0, 0, 0)) -> PostprocessBuffers:
+    """Late fusion of one scene on the GPU with no host sync and no host-side pose: heads of every cav as one batched map each
+    ((n_cav, A, H, W) / (n_cav, 7A, H, W) / (n_cav, A*bins, H, W) or None; or f32 Acts, read from channel `coffsets`), one shared
+    anchor grid (H, W, A, 7) and DEVICE transforms (n_cav, 4, 4) fp32.  Same boxes, order and scores as box_decode_nms_multi
+    over the same cavs in batch order."""
+    c, r = _late_heads(cls_preds, "cls_preds"), _late_heads(reg_preds, "reg_preds")
+    d = _late_heads(dir_preds, "dir_preds") if dir_preds is not None else None
+    oc, orr, od = (int(v) for v in coffsets)
+    n, H, W = c.N, c.H, c.W
+    if not (1 <= n <= 16):
+        raise ValueError(f"box_decode_nms_late: {n} cavs, the call takes 1 to 16")
+    _need_cuda(anchors)
+    if anchors.dtype != torch.float32 or not anchors.is_contiguous() or anchors.dim() != 4 \
+            or tuple(anchors.shape[:2]) != (H, W) or anchors.shape[3] != 7:
+        raise ValueError(f"box_decode_nms_late: anchors must be a contiguous fp32 ({H}, {W}, A, 7) grid")
+    A = anchors.shape[2]
+    for name, a, off, ch in (("cls_preds", c, oc, A), ("reg_preds", r, orr, 7 * A),
+                             ("dir_preds", d, od, A * int(num_bins))):
+        if a is None:
+            continue
+        if (a.N, a.H, a.W) != (n, H, W):
+            raise ValueError(f"box_decode_nms_late: {name} is {(a.N, a.H, a.W)}, cls_preds is {(n, H, W)}")
+        if off < 0 or off + ch > a.C:
+            raise ValueError(f"box_decode_nms_late: {name} needs {ch} channels from offset {off}, it has {a.C}")
+    if not isinstance(transforms, torch.Tensor) or not transforms.is_cuda or transforms.dtype != torch.float32 \
+            or tuple(transforms.shape) != (n, 4, 4) or not transforms.is_contiguous():
+        raise ValueError(f"box_decode_nms_late: transforms must be a contiguous ({n}, 4, 4) fp32 CUDA tensor")
+    if buffers is None:
+        buffers = PostprocessBuffers(H * n, W, A, top, anchors.device)
+    if (buffers.H, buffers.W, buffers.A, buffers.top) != (H * n, W, A, top):
+        raise ValueError("box_decode_nms_late: buffers were made for another geometry")
+    rng = _host_f32(gt_range) if gt_range is not None else None
+    with _Prof("box_decode_nms", 0):
+        _call("heal_box_decode_nms_late", c.view(oc), r.view(orr), d.view(od) if d is not None else None, _p(anchors),
+              _p(transforms), n, H, W, A, float(score_threshold), float(np.float32(dir_offset)), int(num_bins),
+              1 if order == "hwl" else 0, float(nms_threshold), int(top), rng,
+              _p(buffers.boxes), _p(buffers.scores), _p(buffers.count), _p(buffers.stats),
+              _p(buffers.workspace), buffers.workspace.numel())
+    return buffers

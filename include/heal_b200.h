@@ -391,6 +391,19 @@ int heal_box_decode_nms_multi(const heal_cav_heads_t* cavs_host, int n_cav, int 
                               int top, const float* range6_host, float* boxes_out, float* scores_out, int* count_out,
                               int* stats_out, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Late fusion of one scene as a single capturable call: the same decode, filter, sort, rotated NMS and range mask as
+ * heal_box_decode_nms_multi with the cavs in batch order, for cavs that share one anchor grid.  The heads are ONE batched
+ * fp32 channels-last map each: cls (n_cav,H,W,A), reg (n_cav,H,W,7A), dir (n_cav,H,W,A*num_bins) or NULL (channel views with
+ * cstride / coffset, e.g. the three slices of one fused head output).  transforms_dev: DEVICE fp32 (n_cav,4,4) row-major
+ * cav -> ego matrices, read by the decode kernel, so a captured graph picks up new poses.  One decode launch covers every cav.
+ * n_cav <= 16; workspace >= heal_postprocess_workspace(H * n_cav, W, anchors_per_cell, top); boxes, scores, count and stats as
+ * heal_box_decode_nms.  For the same inputs the boxes, their order and the scores equal heal_box_decode_nms_multi's bit for bit. */
+int heal_box_decode_nms_late(const heal_act_t* cls, const heal_act_t* reg, const heal_act_t* dir, const float* anchors,
+                             const float* transforms_dev, int n_cav, int H, int W, int anchors_per_cell,
+                             float score_threshold, float dir_offset, int num_bins, int order_hwl, float nms_threshold,
+                             int top, const float* range6_host, float* boxes_out, float* scores_out, int* count_out,
+                             int* stats_out, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- format conversion between fp32 and (split-)bf16 channels-last buffers ------------------- */
 int heal_act_convert(const heal_act_t* src, const heal_act_t* dst, size_t num_pixels, int channels, void* stream);
 
