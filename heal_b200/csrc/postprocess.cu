@@ -15,6 +15,9 @@
 //                 ordered compaction of the survivors into the output
 // Traps kept: remove_large_pred_bbx takes its "z length" from the y column and only tests it for truthiness (box_utils.py:862-867);
 // IoU is compared as float32; a zero-area union gives NaN and never suppresses.
+// Order: descending score, then ascending candidate slot (cav * H*W*A + (h*W + w)*A + a) on ties -- the stable sort's order.
+// Where the kernel and torch differ by design (NaN logits only): a NaN direction logit never wins the argmax scan (a NaN in bin 0
+// keeps bin 0), and a NaN IoU logit counts as IoU 0 (fmaxf(NaN, 0) = 0, score * 1/16) where torch's clamp would give a NaN score.
 #include <cub/cub.cuh>
 
 #include "common.cuh"
@@ -83,6 +86,7 @@ k_decode(DecP p) {
         const float sx[8] = {1, 1, -1, -1, 1, 1, -1, -1}, sy[8] = {-1, 1, 1, -1, -1, 1, 1, -1}, sz[8] = {-1, -1, -1, -1, 1, 1, 1, 1};
         float c[24];
         float xmin = INFINITY, xmax = -INFINITY, ymin = INFINITY, ymax = -INFINITY, zmin = INFINITY, zmax = -INFINITY;
+        bool has_nan = false;
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
             const float lx = dx * (sx[k] * 0.5f), ly = dy * (sy[k] * 0.5f), lz = dz * (sz[k] * 0.5f);
@@ -93,9 +97,12 @@ k_decode(DecP p) {
             c[3 * k] = X; c[3 * k + 1] = Y; c[3 * k + 2] = Z;
             xmin = fminf(xmin, X); xmax = fmaxf(xmax, X); ymin = fminf(ymin, Y); ymax = fmaxf(ymax, Y);
             zmin = fminf(zmin, Z); zmax = fmaxf(zmax, Z);
+            has_nan = has_nan || isnan(X) || isnan(Y) || isnan(Z);
         }
+        // fminf / fmaxf skip a NaN, torch's max / min return it: a box with a NaN corner (a NaN yaw or size delta) has NaN
+        // lengths in the reference and fails every filter there, so it is dropped here too
         const float xl = xmax - xmin, yl = ymax - ymin;
-        const bool keep = (xl <= 6.f) && (yl <= 6.f) && (yl != 0.f) && (zmin >= -3.f) && (zmax <= 1.f);
+        const bool keep = !has_nan && (xl <= 6.f) && (yl <= 6.f) && (yl != 0.f) && (zmin >= -3.f) && (zmax <= 1.f);
         if (keep) {
             atomicAdd(p.counters + 1, 1);
             key = prob;

@@ -91,6 +91,25 @@ def _host_f32(vals: Sequence[float]):
     return (ctypes.c_float * len(vals))(*[float(np.float32(v)) for v in vals])
 
 
+def _box_range_f32(gt_range: Sequence[float]):
+    """The box range mask's [minx miny minz maxx maxy maxz] as fp32 limits that make the kernel's fp32 test exact.
+    mask_boxes_outside_range_numpy compares fp32 corners with a float64 slice of the range (box_utils.py:415-416).  Each lower
+    limit becomes the smallest fp32 >= it and each upper limit the largest fp32 <= it, so for any fp32 corner c,
+    `c >= lo_f32` is `double(c) >= lo` and `c <= hi_f32` is `double(c) <= hi`.  (Rounding to nearest would keep a corner at
+    float32(-25.6), which lies below -25.6.)"""
+    out = []
+    for k, v in enumerate(gt_range):
+        v = float(v)
+        f = np.float32(v)
+        if k < 3 and float(f) < v:
+            f = np.nextafter(f, np.float32(np.inf))
+        elif k >= 3 and float(f) > v:
+            f = np.nextafter(f, np.float32(-np.inf))
+        out.append(float(f))
+    assert len(out) == 6
+    return (ctypes.c_float * 6)(*out)
+
+
 def _host_i32(vals: Sequence[int]):
     return (ctypes.c_int * len(vals))(*[int(v) for v in vals])
 
@@ -1409,7 +1428,7 @@ def box_decode_nms(cls_preds, reg_preds, dir_preds, anchors: torch.Tensor, trans
         buffers = PostprocessBuffers(H, W, A, top, anchors.device)
     assert (buffers.H, buffers.W, buffers.A, buffers.top) == (H, W, A, top)
     T = _host_f32(np.asarray(torch.as_tensor(transform).detach().cpu().numpy(), dtype=np.float64).reshape(16))
-    rng = _host_f32(gt_range) if gt_range is not None else None
+    rng = _box_range_f32(gt_range) if gt_range is not None else None
     with _Prof("box_decode_nms", 0):
         _call("heal_box_decode_nms", c.view(), r.view(), d.view() if d is not None else None, _p(anchors),
               H, W, A, float(score_threshold), float(np.float32(dir_offset)), int(num_bins), T,
@@ -1457,7 +1476,7 @@ def box_decode_nms_multi(cavs, score_threshold: float, nms_threshold: float, dir
     if buffers is None:
         buffers = PostprocessBuffers(H * n, W, A, top, dev)
     assert (buffers.H, buffers.W, buffers.A, buffers.top) == (H * n, W, A, top)
-    rng = _host_f32(gt_range) if gt_range is not None else None
+    rng = _box_range_f32(gt_range) if gt_range is not None else None
     with _Prof("box_decode_nms", 0):
         _call("heal_box_decode_nms_multi", arr, n, H, W, A, float(score_threshold), float(np.float32(dir_offset)), int(num_bins),
               1 if order == "hwl" else 0, float(nms_threshold), int(top), rng,
@@ -1511,7 +1530,7 @@ def box_decode_nms_late(cls_preds, reg_preds, dir_preds, anchors: torch.Tensor, 
         buffers = PostprocessBuffers(H * n, W, A, top, anchors.device)
     if (buffers.H, buffers.W, buffers.A, buffers.top) != (H * n, W, A, top):
         raise ValueError("box_decode_nms_late: buffers were made for another geometry")
-    rng = _host_f32(gt_range) if gt_range is not None else None
+    rng = _box_range_f32(gt_range) if gt_range is not None else None
     with _Prof("box_decode_nms", 0):
         _call("heal_box_decode_nms_late", c.view(oc), r.view(orr), d.view(od) if d is not None else None, _p(anchors),
               _p(transforms), n, H, W, A, float(score_threshold), float(np.float32(dir_offset)), int(num_bins),

@@ -365,8 +365,15 @@ int heal_sparse_to_bev(const float* feats, const int* coords, const int* rows_de
  * fp64), mask_boxes_outside_range_numpy (:384-421).  Everything stays on the device and on the caller's stream.
  *   cls (1,H,W,A) logits, reg (1,H,W,7A) deltas, dir (1,H,W,A*num_bins) or NULL: fp32 channels-last views (heal_act_t fmt 0)
  *   anchors: device fp32 (H,W,A,7) [x y z h w l yaw] ('hwl' order, order_hwl = 1) or [x y z l w h yaw]
- *   transform4x4_host: row-major cav -> ego matrix; range6_host: [minx miny minz maxx maxy maxz] or NULL (no range mask)
- *   boxes_out (top,8,3) fp32, scores_out (top) fp32 in pick (score) order, count_out: device int = number of boxes written
+ *   transform4x4_host: row-major cav -> ego matrix; range6_host: [minx miny minz maxx maxy maxz] or NULL (no range mask).  A box
+ *     is kept when every corner c has lo <= c <= hi in fp32.  The reference compares fp32 corners with float64 limits, so callers
+ *     pass each lower limit rounded up to the smallest fp32 >= it and each upper limit rounded down to the largest fp32 <= it
+ *     (ops._box_range_f32); the fp32 test is then exactly the float64 one (a corner at float32(-25.6) < -25.6 is dropped).
+ *   boxes_out (top,8,3) fp32, scores_out (top) fp32 in pick (score) order, count_out: device int = number of boxes written.
+ *     Order: descending score, ties by ascending candidate slot, slot = cav * H*W*A + (h*W + w)*A + a (the `top` cut takes the
+ *     first `top` in this order).  The reference's argsort()[::-1] leaves ties in an unspecified order.
+ *   The filters drop a box with any NaN corner, as the reference's NaN lengths do.  Direction logits: the first largest bin
+ *   wins and a NaN never replaces the running best (a NaN in bin 0 keeps bin 0, where torch.max would pick the NaN).
  *   stats_out: device int[2] = anchors above the score threshold, after the size / z filters (NULL allowed)
  *   workspace >= heal_postprocess_workspace(H, W, A, top) bytes; top <= 1320 (the reference uses 1000) */
 size_t heal_postprocess_workspace(int H, int W, int anchors_per_cell, int top);
@@ -378,7 +385,8 @@ int heal_box_decode_nms(const heal_act_t* cls, const heal_act_t* reg, const heal
 
 /* Late fusion / IoU-aware variant (voxel_postprocessor.py:269-376 with several cavs and `iou_preds`): every cav's heads are decoded
  * with ITS transform (cav -> ego) and anchors, the candidates are concatenated in cav order, then ONE filter + sort + rotated NMS
- * + range mask.  `iou` (optional, (1,H,W,A) logits): score *= ((sigmoid(iou) + 1) / 2)^4 after the threshold test (:343-347).
+ * + range mask.  `iou` (optional, (1,H,W,A) logits): score *= ((sigmoid(iou) + 1) / 2)^4 after the threshold test (:343-347); a NaN
+ * IoU logit counts as sigmoid 0 (score * 1/16), where the reference's clamp would give a NaN score.  Order and ties as above.
  * cavs_host: HOST array of n_cav descriptors (all maps H x W x anchors_per_cell); workspace >=
  * heal_postprocess_workspace(H * n_cav, W, anchors_per_cell, top). */
 typedef struct {
