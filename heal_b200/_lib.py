@@ -90,6 +90,7 @@ SIGNATURES = {
     "heal_se_gate": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "heal_pwconv": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     "heal_upsample2x_concat": (_i, [_ap, _ap, _i, _i, _i, _i, _i, _ap, _i, _vp]),
+    "heal_camera_input": (_i, [_vp, _i, _i, _i, _vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
 }
 
 ERRORS = {-1: "HEAL_ERR_ARG", -2: "HEAL_ERR_WORKSPACE", -3: "HEAL_ERR_LAUNCH", -4: "HEAL_ERR_UNSUPPORTED",

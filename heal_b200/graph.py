@@ -237,8 +237,9 @@ class LateFusionGraph:
         out = g.replay()              # out.boxes[:out.count], out.scores[:out.count] on the device, no host sync
 
     `capacities[m]`: for a lidar modality the point capacity of ALL its cavs together (raw clouds, `points` + `agent_offsets`; the
-    live counts travel in the offsets), for a camera modality (cameras, image height, image width) per cav.  The poses are
-    inputs: replaying the graph for another scene uses that scene's transforms."""
+    live counts travel in the offsets), for a camera modality (cameras, image height, image width) per cav for normalised fp32
+    images, or (cameras, frame height, frame width, torch.uint8) for raw uint8 (H0, W0, 3) frames, which the encoder resizes, crops
+    and normalises on the GPU.  The poses are inputs: replaying the graph for another scene uses that scene's transforms."""
 
     CAMERA_KEYS = ("rots", "trans", "intrins", "post_rots", "post_trans")
 
@@ -255,8 +256,13 @@ class LateFusionGraph:
         for m, idx in self.groups.items():
             k = len(idx)
             if model.sensor_type_dict[m] == "camera":
-                cams, h, w = capacities[m]
-                self.inputs[m] = {"imgs": torch.zeros((k, cams, 3, h, w), dtype=torch.float32, device=dev),
+                cams, h, w, *dtype = capacities[m]
+                if dtype and dtype != [torch.uint8]:
+                    raise ValueError(f"{m}: camera capacity {capacities[m]}; (cams, h, w) takes normalised fp32 images and "
+                                     "(cams, H0, W0, torch.uint8) raw frames")
+                imgs = torch.zeros((k, cams, h, w, 3), dtype=torch.uint8, device=dev) if dtype else \
+                    torch.zeros((k, cams, 3, h, w), dtype=torch.float32, device=dev)
+                self.inputs[m] = {"imgs": imgs,
                                   "rots": torch.eye(3, device=dev).repeat(k, cams, 1, 1),
                                   "trans": torch.zeros((k, cams, 3), dtype=torch.float32, device=dev),
                                   "intrins": torch.eye(3, device=dev).repeat(k, cams, 1, 1),
@@ -318,7 +324,8 @@ class LateFusionGraph:
                 for j, i in enumerate(idx):
                     src = batch_data[cavs[i]][f"inputs_{m}"]
                     for k in ("imgs",) + self.CAMERA_KEYS:
-                        buf[k][j].copy_(src[k][0][:, :3] if k == "imgs" else src[k][0], non_blocking=True)
+                        raw = k == "imgs" and buf[k].dtype == torch.uint8         # raw frames (cams, H0, W0, 3) go in whole
+                        buf[k][j].copy_(src[k][0][:, :3] if k == "imgs" and not raw else src[k][0], non_blocking=True)
         T = torch.stack([torch.as_tensor(batch_data[c]['transformation_matrix']).reshape(4, 4).to(torch.float32) for c in cavs])
         self.transforms.copy_(T, non_blocking=True)
 

@@ -39,6 +39,32 @@ def install_gpu_postprocessor():
     return cls
 
 
+CAMERA_DATASETS = (
+    "opencood.data_utils.datasets.intermediate_fusion_dataset",
+    "opencood.data_utils.datasets.intermediate_2stage_fusion_dataset",
+    "opencood.data_utils.datasets.intermediate_heter_fusion_dataset",
+    "opencood.data_utils.datasets.late_fusion_dataset",
+    "opencood.data_utils.datasets.late_heter_fusion_dataset",
+    "opencood.data_utils.datasets.heter_infer.intermediate_heter_infer_fusion_dataset",
+)
+
+
+def install_gpu_camera_input(modules=CAMERA_DATASETS):
+    """Opt-in: rebind `img_transform` and `normalize_img` in the reference's dataset modules that import them, so that the camera
+    branch of an inference batch (flip False, rotate 0, no depth image) carries each decoded frame as a uint8 (H0, W0, 3) tensor
+    with the reference's own post_rot / post_tran; LiftSplatShoot then resizes, crops and normalises every camera of a modality in
+    one heal_camera_input launch.  Every other case runs the reference's functions.  Returns the modules it changed."""
+    from .data_utils.camera_input import reference_pair
+    done = []
+    for name in modules:
+        mod = importlib.import_module(name)
+        ref_t = getattr(mod.img_transform, "reference", mod.img_transform)
+        ref_n = getattr(mod.normalize_img, "reference", mod.normalize_img)
+        mod.img_transform, mod.normalize_img = reference_pair(ref_t, ref_n)
+        done.append(name)
+    return done
+
+
 def install_into_opencood(only=None):
     """Alias the mirrors under their opencood module names (call BEFORE opencood.tools imports the models)."""
     done = []

@@ -178,15 +178,23 @@ class CamEncode_Resnet101(nn.Module):
         y = conv_bn_act(y, blk.conv2, blk.bn2, relu=True)
         return conv_bn_act(y, blk.conv3, blk.bn3, relu=True, residual=idt)
 
-    def heads_nhwc(self, x):
-        """x (BN, 3|4, H, W) fp32 CUDA -> Act f32 (BN, H/8, W/8, D + C): [depth logits | image features] per pixel."""
+    def heads_nhwc(self, x, plan=None):
+        """x (BN, 3|4, H, W) fp32 CUDA -> Act f32 (BN, H/8, W/8, D + C): [depth logits | image features] per pixel.  With a `plan`
+        (data_utils.camera_input.inference_plan), x is raw uint8 frames (BN, H0, W0, 3): heal_camera_input resizes, crops and
+        normalises them straight into the stem's space-to-depth layout."""
         from ..engine import conv_bn_act
-        BN, Cx, H, W = x.shape
-        if (H % 8) or (W % 8):
-            raise NotImplementedError("image sides must be multiples of 8 (the LSS yamls use img_downsample 8)")
-        x4 = torch.zeros((BN, 4, H, W), dtype=torch.float32, device=x.device)
-        x4[:, :3] = x[:, :3]
-        a = ops.to_act(torch.nn.functional.pixel_unshuffle(x4, 4))          # (BN, H/4, W/4, 64): layout plumbing of the raw image
+        if plan is not None:
+            H, W = plan.final_dim
+            if (H % 8) or (W % 8):
+                raise NotImplementedError("image sides must be multiples of 8 (the LSS yamls use img_downsample 8)")
+            a = ops.camera_input(x, plan, "s2d")                                # (BN, H/4, W/4, 64)
+        else:
+            BN, Cx, H, W = x.shape
+            if (H % 8) or (W % 8):
+                raise NotImplementedError("image sides must be multiples of 8 (the LSS yamls use img_downsample 8)")
+            x4 = torch.zeros((BN, 4, H, W), dtype=torch.float32, device=x.device)
+            x4[:, :3] = x[:, :3]
+            a = ops.to_act(torch.nn.functional.pixel_unshuffle(x4, 4))      # (BN, H/4, W/4, 64): layout plumbing of the raw image
         y = conv_bn_act(a, self._stem_as_s2d_conv(), None, relu=True)         # phase-major (BN, H/4, W/4, 4*64) = logical (BN, H/2, W/2, 64)
         y = ops.maxpool3x3s2(y, depth_to_space_in=True)                       # (BN, H/4, W/4, 64)
         for blk in self.layer1:
@@ -285,9 +293,13 @@ class CamEncode(nn.Module):
 
     _fused_heads = CamEncode_Resnet101._fused_heads
 
-    def heads_nhwc(self, x):
-        """x (BN, 3|4, H, W) fp32 CUDA -> Act f32 (BN, H/ds, W/ds, D + C): [depth logits | image features] per pixel."""
+    def heads_nhwc(self, x, plan=None):
+        """x (BN, 3|4, H, W) fp32 CUDA -> Act f32 (BN, H/ds, W/ds, D + C): [depth logits | image features] per pixel.  With a `plan`
+        (data_utils.camera_input.inference_plan), x is raw uint8 frames (BN, H0, W0, 3), resized, cropped and normalised to NCHW fp32
+        by heal_camera_input first."""
         from ..engine import conv_bn_act
+        if plan is not None:
+            x = ops.camera_input(x, plan, "nchw")
         self._check_sides(x.shape[2], x.shape[3])
         r3, r4, r5 = self.trunk.endpoints_nhwc(x.float().contiguous())
         f = self.up1.forward_nhwc(r5, r4)
@@ -351,6 +363,15 @@ class LiftSplatShoot(nn.Module):
         return ops.lss_cell_index(self.frustum, post_inv, post_trans.reshape(B * N, 3), combine, trans.reshape(B * N, 3),
                                   self._lower_host, self._dx_host, self._nx_host)
 
+    def camera_plan(self, H0, W0):
+        """The reference's inference resize / crop of a raw (H0, W0) frame for this encoder's data_aug_conf (cached per size).  The
+        batch's post_rots / post_trans are still what the geometry uses."""
+        from ..data_utils.camera_input import inference_plan
+        plans = self.__dict__.setdefault("_camera_plans", {})
+        if (H0, W0) not in plans:
+            plans[(H0, W0)] = inference_plan(self.data_aug_conf, H0, W0)
+        return plans[(H0, W0)]
+
     def forward_act(self, data_dict, modality_name, fmt=None):
         """image trunk + heads on the conv engine -> frustum cell index -> deterministic sorted BEV pooling
         (heal_lss_pool_sorted reads logits and features straight from the fused heads' channels-last output)."""
@@ -358,13 +379,20 @@ class LiftSplatShoot(nn.Module):
         require_eval(self)
         d = data_dict[f'inputs_{modality_name}']
         x = d['imgs']
-        B, N, C, imH, imW = x.shape
+        plan = None
+        if x.dtype == torch.uint8:                                        # raw sensor frames (B, N, H0, W0, 3), resampled on the GPU
+            B, N, H0, W0, _ = x.shape
+            plan = self.camera_plan(H0, W0)
+            x = x.reshape(B * N, H0, W0, 3)
+        else:                                                             # images the reference's DataLoader already normalised
+            B, N, C, imH, imW = x.shape
+            x = x.view(B * N, C, imH, imW)
         if _os.environ.get("HEAL_CAM_TRUNK_TORCH", "0") == "1":           # A/B hook: torch / cuDNN trunk + atomic pooling (round 1)
-            depth_logits, feat = self.camencode.heads(x.view(B * N, C, imH, imW))
+            depth_logits, feat = self.camencode.heads(x if plan is None else ops.camera_input(x, plan, "nchw"))
             if self.depth_supervision:
                 self.depth_items = (depth_logits, None)
             return self.bev_from_heads(depth_logits, feat, d['rots'], d['trans'], d['intrins'], d['post_rots'], d['post_trans'])
-        y = self.camencode.heads_nhwc(x.view(B * N, C, imH, imW))         # Act f32 (BN, fH, fW, D + camC)
+        y = self.camencode.heads_nhwc(x, plan)                            # Act f32 (BN, fH, fW, D + camC)
         D, camC, fH, fW = self.D, self.camC, y.H, y.W
         S, HW = D + camC, y.H * y.W
         if self.depth_supervision:

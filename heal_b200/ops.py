@@ -1118,6 +1118,49 @@ def upsample2x_concat(x1: Act, x2: Act, out_fmt: str) -> Act:
 
 
 # ------------------------------------------------------------------------------------------------
+# camera input (csrc/camera_input.cu): raw uint8 frames -> the reference's inference resize, crop and normalisation
+# ------------------------------------------------------------------------------------------------
+CAMERA_LAYOUTS = {"nchw": 0, "s2d": 1}
+
+
+@_guard
+def camera_input(frames: torch.Tensor, plan, layout: str = "nchw"):
+    """frames uint8 (n, H0, W0, 3) CUDA, HWC as decoded; plan = data_utils.camera_input.inference_plan(conf, H0, W0).
+    layout 'nchw' -> fp32 (n, 3, fH, fW), what normalize_img returns per frame (CamEncode's input);
+    layout 's2d'  -> Act f32 (n, fH/4, fW/4, 64), channel c*16 + dy*4 + dx with c == 3 zero: pixel_unshuffle(image with a zero 4th
+                     plane, 4), the ResNet-101 stem's space-to-depth input."""
+    if not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8:
+        raise TypeError(f"camera_input: frames must be a uint8 tensor, got {getattr(frames, 'dtype', type(frames))}")
+    if frames.dim() != 4 or frames.shape[3] != 3:
+        raise ValueError(f"camera_input: frames must be (n, H0, W0, 3) RGB, got {tuple(frames.shape)}")
+    if not frames.is_contiguous():
+        raise ValueError("camera_input: frames must be contiguous")
+    if layout not in CAMERA_LAYOUTS:
+        raise ValueError(f"camera_input: layout '{layout}', expected one of {sorted(CAMERA_LAYOUTS)}")
+    n, H0, W0, _ = frames.shape
+    if (H0, W0) != (plan.H0, plan.W0):
+        raise ValueError(f"camera_input: frames are {H0}x{W0}, the plan was made for {plan.H0}x{plan.W0}")
+    fH, fW = plan.final_dim
+    l, t, r, b = plan.crop
+    if (b - t, r - l) != (fH, fW):
+        raise ValueError(f"camera_input: crop {plan.crop} is {b - t}x{r - l}, final_dim is {fH}x{fW}")
+    if layout == "s2d" and (fH % 8 or fW % 8):
+        raise ValueError(f"camera_input: the space-to-depth layout needs sides that are multiples of 8, final_dim is {fH}x{fW}")
+    _need_cuda(frames)
+    cols, ck, rows, rk, span = plan.tables(frames.device)
+    if layout == "nchw":
+        out = torch.empty((n, 3, fH, fW), dtype=torch.float32, device=frames.device)
+        res = out
+    else:
+        res = act_empty(n, fH // 4, fW // 4, 64, "f32", frames.device)
+        out = res.t
+    with _Prof("camera_input", 0, float(n) * H0 * W0 * 3 + 4.0 * out.numel()):
+        _call("heal_camera_input", _p(frames), n, H0, W0, _p(cols), ck, _p(rows), rk, fH, fW, span, CAMERA_LAYOUTS[layout],
+              _p(out))
+    return res
+
+
+# ------------------------------------------------------------------------------------------------
 # sparse 3-D convolution (SECOND)
 # ------------------------------------------------------------------------------------------------
 class SparseTensor:

@@ -479,6 +479,24 @@ int heal_mask_points(const float* points, const int* perm, const int* agent_offs
                      const float* range6_host, int remove_ego, float* points_out, int* agent_offsets_out,
                      void* workspace, size_t workspace_bytes, void* stream);
 
+/* The camera agent's image stage (SURVEY.md 8f-4): the reference's inference resize, crop and normalisation, done per camera on
+ * the host in its DataLoader workers (intermediate_heter_fusion_dataset.py:199-246; camera_utils.py:33-59 sample_augmentation
+ * with is_train False, :62-91 img_transform = PIL resize with its default antialiased bicubic filter, then crop; :120-125
+ * normalize_img = ToTensor + Normalize(ImageNet mean / std)).  Bit-exact: Pillow's 8-bit fixed-point resample (horizontal pass,
+ * clipped to uint8, then vertical pass), black outside the resized frame, then (u / 255 - mean) / std in fp32.
+ *   frames      (n_img, H0, W0, 3) uint8, HWC as decoded; every camera of every agent of one modality in one call
+ *   col_table   (fW, 2 + col_taps) i32: per output column, the first source column, the tap count and col_taps int32 taps
+ *               (1 << 22 = 1.0); entry i is column crop_left + i of the resized frame, so the crop box is folded into the table
+ *               and a count of 0 marks a column outside the resized frame.  An axis that keeps its size has one tap of 1 << 22.
+ *   row_table   (fH, 2 + row_taps) i32: the same per output row
+ *   span_rows   the most source rows one 32-row band of output rows needs (sizes the shared tile; the host computes it)
+ *   layout 0    out (n_img, 3, fH, fW) fp32 NCHW (heal_stem_conv_swish reads it)
+ *   layout 1    out (n_img, fH/4, fW/4, 64) fp32 channels-last, channel c*16 + dy*4 + dx, c == 3 zero: the space-to-depth input of
+ *               the ResNet-101 stem (fH, fW multiples of 8)
+ * No atomics, no host sync: the same bits on every run. */
+int heal_camera_input(const uint8_t* frames, int n_img, int H0, int W0, const int* col_table, int col_taps,
+                      const int* row_table, int row_taps, int fH, int fW, int span_rows, int layout, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
