@@ -21,6 +21,7 @@
 #include <cub/cub.cuh>
 
 #include "common.cuh"
+#include "quad_iou.cuh"
 #include "../../include/heal_b200.h"
 
 namespace {
@@ -139,54 +140,7 @@ __global__ void k_gather_top(const float* __restrict__ keys_sorted, const int* _
             in = in && (c[3 * k] >= lx) && (c[3 * k] <= hx) && (c[3 * k + 1] >= ly) && (c[3 * k + 1] <= hy) && (c[3 * k + 2] >= lz) && (c[3 * k + 2] <= hz);
     }
     inrange[r] = in ? 1 : 0;
-    double x[4], y[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) { x[k] = (double)c[3 * k]; y[k] = (double)c[3 * k + 1]; }
-    double a2 = 0.0;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) a2 += x[k] * y[(k + 1) & 3] - y[k] * x[(k + 1) & 3];
-    double* o = poly + (size_t)r * 9;
-    if (a2 < 0.0) {                       // clockwise -> reverse (oracle: p[::-1])
-#pragma unroll
-        for (int k = 0; k < 4; ++k) { o[2 * k] = x[3 - k]; o[2 * k + 1] = y[3 - k]; }
-    } else {
-#pragma unroll
-        for (int k = 0; k < 4; ++k) { o[2 * k] = x[k]; o[2 * k + 1] = y[k]; }
-    }
-    o[8] = fabs(0.5 * a2);
-}
-
-__device__ __forceinline__ double poly_area2(const double* px, const double* py, int n) {
-    double s = 0.0;
-    for (int k = 0; k < n; ++k) { const int k1 = (k + 1 == n) ? 0 : k + 1; s += px[k] * py[k1] - py[k] * px[k1]; }
-    return s;
-}
-
-// intersection area of two counter-clockwise convex quads: clip P against the 4 directed edges of Q (keep the left side)
-__device__ double quad_intersection(const double* P, const double* Q) {
-    double ax[10], ay[10], bx[10], by[10];
-    int n = 4;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) { ax[k] = P[2 * k]; ay[k] = P[2 * k + 1]; }
-    for (int e = 0; e < 4; ++e) {
-        const double qx = Q[2 * e], qy = Q[2 * e + 1];
-        const double ex = Q[2 * ((e + 1) & 3)] - qx, ey = Q[2 * ((e + 1) & 3) + 1] - qy;
-        int m = 0;
-        for (int k = 0; k < n; ++k) {
-            const int k1 = (k + 1 == n) ? 0 : k + 1;
-            const double sp = ex * (ay[k] - qy) - ey * (ax[k] - qx);
-            const double sq = ex * (ay[k1] - qy) - ey * (ax[k1] - qx);
-            if (sp >= 0.0) { bx[m] = ax[k]; by[m] = ay[k]; ++m; }
-            if ((sp > 0.0 && sq < 0.0) || (sp < 0.0 && sq > 0.0)) {
-                const double t = sp / (sp - sq);
-                bx[m] = ax[k] + t * (ax[k1] - ax[k]); by[m] = ay[k] + t * (ay[k1] - ay[k]); ++m;
-            }
-        }
-        n = m;
-        if (n < 3) return 0.0;
-        for (int k = 0; k < n; ++k) { ax[k] = bx[k]; ay[k] = by[k]; }
-    }
-    return fabs(0.5 * poly_area2(ax, ay, n));
+    quad_ccw(c, poly + (size_t)r * 9);
 }
 
 __global__ void __launch_bounds__(64)

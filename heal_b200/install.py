@@ -65,6 +65,20 @@ def install_gpu_camera_input(modules=CAMERA_DATASETS):
     return done
 
 
+def install_gpu_eval():
+    """Opt-in: rebind `opencood.utils.eval_utils.caluclate_tp_fp` to heal_b200.utils.eval_utils.caluclate_tp_fp, which matches a
+    frame's detections to its GT boxes on the GPU when both are CUDA fp32 (N, 8, 3) tensors and calls the reference function
+    (kept as `.reference`) otherwise.  inference.py, inference_w_noise.py and inference_heter_in_order.py all call it through the
+    module, so this covers the three.  Returns the new function."""
+    from .utils import eval_utils as ours
+    mod = importlib.import_module("opencood.utils.eval_utils")
+    cur = mod.caluclate_tp_fp
+    if cur is not ours.caluclate_tp_fp:
+        ours.caluclate_tp_fp.reference = cur
+    mod.caluclate_tp_fp = ours.caluclate_tp_fp
+    return ours.caluclate_tp_fp
+
+
 def install_into_opencood(only=None):
     """Alias the mirrors under their opencood module names (call BEFORE opencood.tools imports the models)."""
     done = []

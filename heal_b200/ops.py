@@ -1581,3 +1581,70 @@ def box_decode_nms_late(cls_preds, reg_preds, dir_preds, anchors: torch.Tensor, 
               _p(buffers.boxes), _p(buffers.scores), _p(buffers.count), _p(buffers.stats),
               _p(buffers.workspace), buffers.workspace.numel())
     return buffers
+
+
+# ------------------------------------------------------------------------------------------------
+# detection evaluation (csrc/eval.cu): the TP / FP matching of eval_utils.caluclate_tp_fp for one frame
+# ------------------------------------------------------------------------------------------------
+class EvalBuffers:
+    """Caller-owned outputs + workspace of heal_eval_tp_fp, reusable for every frame of at most K detections and G GT boxes.
+    The outputs of a call share one byte buffer, `packed` = [status int32 | K sorted scores fp32 | (n_thr, K) TP flags uint8],
+    so one device-to-host copy brings all three back (`unpack`)."""
+
+    def __init__(self, K: int, G: int, device):
+        self.K, self.G = int(K), int(G)
+        nbytes = int(lib.heal_eval_workspace(self.K, self.G))
+        if nbytes == 0:
+            raise ValueError(f"bad evaluation sizes K={K}, G={G}")
+        self.workspace = torch.empty((nbytes,), dtype=torch.uint8, device=device)
+        self.out = torch.empty((4 + 4 * self.K + 8 * self.K,), dtype=torch.uint8, device=device)
+        self._bind(0, 1)
+
+    def _bind(self, K: int, n_thr: int):
+        n = 4 + 4 * K + n_thr * K
+        self.packed = self.out[:n]
+        self.status = self.out[:4].view(torch.int32)
+        self.scores = self.out[4:4 + 4 * K].view(torch.float32)
+        self.tp = self.out[4 + 4 * K:n].view(n_thr, K)
+
+    @staticmethod
+    def unpack(packed: torch.Tensor, K: int, n_thr: int):
+        """`packed` (a copy of .packed, on any device) -> (status int, scores (K,) fp32, tp (n_thr, K) uint8)."""
+        return (int(packed[:4].view(torch.int32)[0]), packed[4:4 + 4 * K].view(torch.float32),
+                packed[4 + 4 * K:4 + 4 * K + n_thr * K].view(n_thr, K))
+
+
+def _eval_boxes(t, name: str) -> torch.Tensor:
+    if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or t.dim() != 3 or tuple(t.shape[1:]) != (8, 3):
+        raise ValueError(f"eval_tp_fp: {name} must be a (N, 8, 3) fp32 tensor")
+    _need_cuda(t)
+    if not t.is_contiguous():
+        raise ValueError(f"eval_tp_fp: {name} must be contiguous")
+    return t
+
+
+@_guard
+def eval_tp_fp(det: torch.Tensor, scores: torch.Tensor, gt: torch.Tensor, thresholds: Sequence[float],
+               buffers: Optional[EvalBuffers] = None) -> EvalBuffers:
+    """eval_utils.caluclate_tp_fp for one frame at up to 8 IoU thresholds, on the GPU with no host sync: det (K, 8, 3), scores (K,)
+    and gt (G, 8, 3) fp32 CUDA tensors.  Returns the buffers with .scores (K,) fp32 in descending order (ties by ascending index),
+    .tp (n_thr, K) uint8 flags in that order (FP = 1 - TP) and .status (1,) int32 (bit HEAL_EVAL_ZERO_UNION = 1: a union of area
+    0, where the reference raises ZeroDivisionError).  The rules are those of include/heal_b200.h.  Buffers too small for K or G
+    are replaced by larger ones: keep the returned object for the next frame."""
+    _eval_boxes(det, "det")
+    _eval_boxes(gt, "gt")
+    K, G = det.shape[0], gt.shape[0]
+    if not isinstance(scores, torch.Tensor) or scores.dtype != torch.float32 or tuple(scores.shape) != (K,) \
+            or not scores.is_contiguous():
+        raise ValueError(f"eval_tp_fp: scores must be a contiguous ({K},) fp32 tensor")
+    _need_cuda(scores)
+    if scores.device != det.device or gt.device != det.device:
+        raise ValueError("eval_tp_fp: det, scores and gt must be on one device")
+    thr = [float(v) for v in thresholds]
+    if buffers is None or buffers.K < K or buffers.G < G:
+        buffers = EvalBuffers(max(K, buffers.K if buffers else 0), max(G, buffers.G if buffers else 0), det.device)
+    with _Prof("eval_tp_fp", 0, 24.0 * 4 * (K + G) + 4.0 * K * G * (1 + len(thr)) + (4.0 + len(thr)) * K):
+        _call("heal_eval_tp_fp", _p(det), _p(scores), K, _p(gt), G, _host_f32(thr), len(thr), _p(buffers.out[4:]),
+              _p(buffers.out[4 + 4 * K:]), _p(buffers.out), _p(buffers.workspace), buffers.workspace.numel())
+    buffers._bind(K, len(thr))
+    return buffers

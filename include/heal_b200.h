@@ -412,6 +412,32 @@ int heal_box_decode_nms_late(const heal_act_t* cls, const heal_act_t* reg, const
                              int top, const float* range6_host, float* boxes_out, float* scores_out, int* count_out,
                              int* stats_out, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- detection evaluation: true / false positives of one frame ------------------------------------------------------
+ * replaces eval_utils.caluclate_tp_fp (opencood/utils/eval_utils.py:40-92), which opencood/tools/inference.py:171-185 (and
+ * inference_w_noise.py, inference_heter_in_order.py) calls once per frame for each of IoU 0.3, 0.5 and 0.7; one call here does up
+ * to 8 thresholds.
+ *   det_corners (K,8,3) fp32, det_scores (K) fp32, gt_corners (G,8,3) fp32: device.  Only corners 0..3, x and y, are used: the
+ *     shapely Polygon of convert_format (common_utils.py:255-270), in fp64 and made counter-clockwise.
+ *   thresholds_host: n_thr fp32 IoU thresholds, each > 0.
+ *   sorted_scores_out (K) fp32: the scores in descending order.  Ties go by ascending input index (a stable sort) and NaN scores
+ *     last.  The reference's np.argsort(-det_score) leaves the order of tied scores unspecified (NumPy's default sort is not
+ *     stable and its SIMD dispatch depends on the CPU); this is the one place where the result can differ from the reference's.
+ *   tp_out (n_thr, K) uint8: 1 = TP, 0 = FP, per threshold and sorted detection.
+ *   status_out: device int, HEAL_EVAL_ZERO_UNION set when a det and a GT have a union of area 0 (two degenerate boxes), where the
+ *     reference's compute_iou raises ZeroDivisionError; the flags are then meaningless.
+ * Rules, as the reference with NumPy 2: IoU = inter / (area_det + area_gt - inter) in fp64, the det clipped against the GT's
+ * edges, rounded once to fp32 (compute_iou, common_utils.py:250-252); boxes whose bounding boxes do not touch have IoU 0.  Dets
+ * are taken in score order; a det is FP when no GT is left or when the largest fp32 IoU over the GTs left is below the threshold
+ * compared in fp32 (NEP 50 casts the Python float to the array's float32, so an IoU equal to float32(0.7) < 0.7 is a TP; NumPy 1
+ * compared in float64), else TP and it takes the GT of that IoU, the lowest GT index on equal IoUs (np.argmax + list.pop).
+ * K <= 4096, G <= 4096, 1 <= n_thr <= 8, else HEAL_ERR_ARG.  K = 0 launches nothing (status_out is cleared); G = 0 makes every
+ * det FP.  workspace >= heal_eval_workspace(K, G) bytes. */
+#define HEAL_EVAL_ZERO_UNION 1
+size_t heal_eval_workspace(int K, int G);
+int heal_eval_tp_fp(const float* det_corners, const float* det_scores, int K, const float* gt_corners, int G,
+                    const float* thresholds_host, int n_thr, float* sorted_scores_out, unsigned char* tp_out, int* status_out,
+                    void* ws, size_t ws_bytes, void* stream);
+
 /* ---- format conversion between fp32 and (split-)bf16 channels-last buffers ------------------- */
 int heal_act_convert(const heal_act_t* src, const heal_act_t* dst, size_t num_pixels, int channels, void* stream);
 
