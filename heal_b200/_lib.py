@@ -50,6 +50,7 @@ SIGNATURES = {
     "heal_warp_affine": (_i, [_ap, _vp, _vp, _i, _i, _i, _i, _ap, _vp]),
     "heal_v2v_aggregate": (_i, [_ap, _ap, _ap, _vp, _vp, _i, _i, _i, _i, _i, _i, _ap, _vp]),
     "heal_gru_gate": (_i, [_ap, _c.c_longlong, _i, _ap, _vp]),
+    "heal_ego_mha": (_i, [_ap, _ap, _vp, _vp, _vp, _i, _i, _i, _i, _i, _ap, _vp]),
     "heal_swap_attention": (_i, [_ap, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _ap, _vp]),
     "heal_mean_layernorm": (_i, [_ap, _i, _i, _i, _i, _i, _vp, _vp, _c.c_float, _ap, _vp]),
     "heal_window_attention": (_i, [_ap, _i, _i, _i, _i, _i, _i, _vp, _ap, _vp]),

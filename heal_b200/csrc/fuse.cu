@@ -629,6 +629,76 @@ __global__ void __launch_bounds__(256) k_gru_gate(ActV zc, ActV out, long long n
     act_store4(out, pix, c, h);
 }
 
+// ---- Where2commFusion attention core (fusion_in_one.py:431-484, where2comm_attn.py:64-103) ---------------------------------
+// nn.MultiheadAttention with one query (the warped ego) over the scene's n warped agents, per pixel and head.  The k | v in-
+// projection is a per-pixel linear map, so it commutes with the bilinear warp (zero-padded taps contribute nothing): the
+// kernel samples the projection of the UNWARPED maps and adds the bias afterwards.
+constexpr int MHA_C = 256;         // embed dim (every baseline yaml has in_head 256)
+constexpr int MHA_HEADS = 8;       // EncodeLayer's n_head; dim_head 32 = 8 lanes of 4 channels
+constexpr int MHA_PIX = 256 / (MHA_C / 4);      // pixels per 256-thread block
+constexpr int MHA_SCENES = 64;     // scenes per heal_ego_mha launch (their agent ranges travel in the parameter block)
+
+struct MhaP {
+    ActV q, kv, out; const float* kv_bias; const double* theta;
+    int H, W, b0;
+    float scale;
+    int2 scene[MHA_SCENES];        // (first kv / theta image, agents n) of scene b0 + blockIdx.y
+};
+
+// thread = (pixel, 4 channels); the 8 lanes of a head reduce q.k by shuffles, and a warp never spans two pixels.  The taps of
+// the block's (pixel, agent) pairs are computed once into shared memory; each agent's sampled k and v stay in registers.
+__global__ void __launch_bounds__(256) k_ego_mha(MhaP p) {
+    __shared__ Tap sTap[MHA_PIX][MAX_AGENTS];
+    const int HW = p.H * p.W;
+    const int b = p.b0 + blockIdx.y, first = p.scene[blockIdx.y].x, n = p.scene[blockIdx.y].y;
+    const int pix0 = blockIdx.x * MHA_PIX;
+    for (int it = threadIdx.x; it < MHA_PIX * n; it += blockDim.x) {
+        const int lp = it / n, j = it % n, pix = pix0 + lp;
+        if (pix < HW) sTap[lp][j] = make_tap(p.theta + 6 * (long long)(first + j), pix / p.W, pix % p.W, p.H, p.W, 0);
+    }
+    __syncthreads();
+    const int lp = threadIdx.x / (MHA_C / 4), pix = pix0 + lp;
+    if (pix >= HW) return;                                           // whole warps: 32 threads share one pixel
+    const int c = (threadIdx.x % (MHA_C / 4)) * 4;
+    float4 qv = act_load4(p.q, (size_t)b * HW + pix, c);
+    qv.x *= p.scale; qv.y *= p.scale; qv.z *= p.scale; qv.w *= p.scale;
+    const float4 bk = __ldg(reinterpret_cast<const float4*>(p.kv_bias + c));
+    const float4 bv = __ldg(reinterpret_cast<const float4*>(p.kv_bias + MHA_C + c));
+    float4 v[MAX_AGENTS];
+    float s[MAX_AGENTS];
+    float m = -INFINITY;
+#pragma unroll
+    for (int j = 0; j < MAX_AGENTS; ++j) {
+        if (j < n) {
+            const Tap t = sTap[lp][j];
+            const long long img0 = (long long)(first + j) * HW;
+            float4 k = tap_sample4(p.kv, img0, t, c);
+            v[j] = tap_sample4(p.kv, img0, t, MHA_C + c);
+            k.x += bk.x; k.y += bk.y; k.z += bk.z; k.w += bk.w;
+            v[j].x += bv.x; v[j].y += bv.y; v[j].z += bv.z; v[j].w += bv.w;
+            float d = qv.x * k.x + qv.y * k.y + qv.z * k.z + qv.w * k.w;
+            d += __shfl_xor_sync(0xffffffffu, d, 1);
+            d += __shfl_xor_sync(0xffffffffu, d, 2);
+            d += __shfl_xor_sync(0xffffffffu, d, 4);
+            s[j] = d;
+            m = fmaxf(m, d);
+        }
+    }
+    float sum = 0.f;
+#pragma unroll
+    for (int j = 0; j < MAX_AGENTS; ++j) if (j < n) { s[j] = expf(s[j] - m); sum += s[j]; }
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int j = 0; j < MAX_AGENTS; ++j) {
+        if (j < n) {
+            const float a = s[j] / sum;
+            acc.x = fmaf(a, v[j].x, acc.x); acc.y = fmaf(a, v[j].y, acc.y);
+            acc.z = fmaf(a, v[j].z, acc.z); acc.w = fmaf(a, v[j].w, acc.w);
+        }
+    }
+    act_store4(p.out, (size_t)b * HW + pix, c, acc);
+}
+
 }  // namespace
 
 static inline ActV to_view(const heal_act_t* a) {
@@ -786,6 +856,36 @@ extern "C" int heal_v2v_aggregate(const heal_act_t* q, const heal_act_t* p_node,
             p.node[y] = make_int4(nd[0], nd[1], nd[2], nd[3]);
         }
         k_v2v_aggregate<<<dim3((unsigned)grid_x(H, W, C), nb), 256, 0, (cudaStream_t)stream_>>>(p);
+        ++launches;
+    }
+    return heal_check_launch(launches);
+}
+
+extern "C" int heal_ego_mha(const heal_act_t* q, const heal_act_t* kv, const float* kv_bias, const double* theta,
+                            const int* n_agents_host, int B, int H, int W, int C, int heads, const heal_act_t* out,
+                            void* stream_) {
+    if (!q || !q->data || !kv || !kv->data || !kv_bias || !theta || !n_agents_host || !out || !out->data) return HEAL_ERR_ARG;
+    if (B < 0 || H < 1 || W < 1 || q->fmt < 0 || q->fmt > 2 || kv->fmt < 0 || kv->fmt > 2 || out->fmt < 0 || out->fmt > 2)
+        return HEAL_ERR_ARG;
+    if (C != MHA_C || heads != MHA_HEADS) return HEAL_ERR_UNSUPPORTED;
+    if (!aligned4(q) || !aligned4(kv) || !aligned4(out) || ((uintptr_t)kv_bias & 15)) return HEAL_ERR_UNSUPPORTED;
+    if ((long long)H * W >= (1LL << 31)) return HEAL_ERR_UNSUPPORTED;      // pixel indices are ints
+    for (int b = 0; b < B; ++b)          // every count before the first launch, so a bad one leaves the output untouched
+        if (n_agents_host[b] < 1 || n_agents_host[b] > MAX_AGENTS) return HEAL_ERR_ARG;
+    MhaP p;
+    p.q = to_view(q); p.kv = to_view(kv); p.out = to_view(out); p.kv_bias = kv_bias; p.theta = theta;
+    p.H = H; p.W = W;
+    p.scale = (float)sqrt(1.0 / (double)(C / heads));      // PyTorch's q * sqrt(1 / dim_head), in fp32
+    const unsigned grid = (unsigned)(((long long)H * W + MHA_PIX - 1) / MHA_PIX);
+    int first = 0, launches = 0;
+    for (int b0 = 0; b0 < B; b0 += MHA_SCENES) {
+        const int nb = B - b0 < MHA_SCENES ? B - b0 : MHA_SCENES;
+        p.b0 = b0;
+        for (int z = 0; z < nb; ++z) {
+            p.scene[z] = make_int2(first, n_agents_host[b0 + z]);
+            first += n_agents_host[b0 + z];
+        }
+        k_ego_mha<<<dim3(grid, (unsigned)nb), 256, 0, (cudaStream_t)stream_>>>(p);
         ++launches;
     }
     return heal_check_launch(launches);

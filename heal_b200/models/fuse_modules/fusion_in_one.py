@@ -1,8 +1,7 @@
 """Fusion operator mirrors of opencood/models/fuse_modules/fusion_in_one.py: AttFusion (:126-151), MaxFusion (:87-124),
-V2VNetFusion (:203-318), V2XViTFusion (:320-372) and CoBEVT (:374-429), with the reference's `forward(x, record_len,
-affine_matrix)` signature (NCHW) and `forward_nhwc` (conv-engine activations).  DiscoFusion cannot be constructed in the
-reference (it imports a `disco_fuse` module the reference does not ship); Where2comm and Who2com are out of scope (SURVEY.md 2.1
-row 14)."""
+V2VNetFusion (:203-318), V2XViTFusion (:320-372), CoBEVT (:374-429), Where2commFusion (:431-484) and Who2comFusion (:486-539),
+with the reference's `forward(x, record_len, affine_matrix)` signature (NCHW) and `forward_nhwc` (conv-engine activations).
+DiscoFusion cannot be constructed in the reference (it imports a `disco_fuse` module the reference does not ship)."""
 import numpy as np
 import torch
 import torch.nn as nn
@@ -323,6 +322,122 @@ class CoBEVT(nn.Module):
     def forward(self, x, record_len, affine_matrix):
         require_eval(self)
         self._check(x.shape[1], x.shape[2], x.shape[3], affine_matrix.shape[1])
+        return ops.act_to_nchw(self.forward_nhwc(ops.to_act(x), record_len, affine_matrix))
+
+
+class EncodeLayer(nn.Module):
+    """Parameter container of where2comm_attn.py:64-103 (keys attn.{in_proj_weight, in_proj_bias, out_proj.*}, linear{1,2}.*,
+    norm{1,2}.*); Where2commFusion runs it."""
+
+    def __init__(self, channels, n_head=8, dropout=0):
+        super().__init__()
+        self.attn = nn.MultiheadAttention(channels, n_head, dropout)
+        self.linear1 = nn.Linear(channels, channels)
+        self.linear2 = nn.Linear(channels, channels)
+        self.norm1 = nn.LayerNorm(channels)
+        self.norm2 = nn.LayerNorm(channels)
+
+
+def _linear_conv(lin):
+    return _conv_from(lin.weight.detach()[:, :, None, None], None if lin.bias is None else lin.bias.detach(), 0)
+
+
+class Where2commFusion(nn.Module):
+    """Where2comm's fusion (fusion_in_one.py:431-484) with the reference's ctor and state-dict keys (`mha_fusion.*`).
+
+    Per scene, EncodeLayer runs with the warped ego X_0 as the one query over the n_b warped agents X_j, per pixel:
+    y1 = LN1(X_0 + out_proj(MHA)), out = LN2(y1 + linear2(ReLU(linear1(y1)))).  The k | v in-projection commutes with the
+    warp, so it runs as one bias-free 1x1 conv on the UNWARPED maps and heal_ego_mha samples it (adding the bias afterwards):
+        warp the egos (heal_warp_affine) -> q 1x1 conv (+ b_q) -> k|v 1x1 conv on x -> heal_ego_mha
+        -> out_proj 1x1 conv + X_0 -> heal_mean_layernorm -> linear1 + ReLU -> linear2 + y1 -> heal_mean_layernorm.
+    The packed convs and the k|v bias are a derived cache, rebuilt when a parameter changes."""
+
+    def __init__(self, feature_dims):
+        super().__init__()
+        self.mha_fusion = EncodeLayer(feature_dims)
+        self.feature_dims = feature_dims
+        self._derived = None
+
+    def _check(self, C):
+        if C != self.feature_dims:
+            raise ValueError(f"Where2commFusion: feature_dims is {self.feature_dims} but the feature map has {C} channels")
+        if C != 256 or self.mha_fusion.attn.num_heads != 8:
+            raise NotImplementedError(f"Where2commFusion: heal_ego_mha implements 256 channels in 8 heads (every shipped "
+                                      f"config), not {C}")
+
+    def _packed(self):
+        enc = self.mha_fusion
+        sig = engine._sig(*enc.modules())
+        if self._derived is None or self._derived[0] != sig:
+            C = self.feature_dims
+            w, b = enc.attn.in_proj_weight.detach(), enc.attn.in_proj_bias.detach()
+            q = _conv_from(w[:C, :, None, None], b[:C], 0)
+            kv = _conv_from(w[C:, :, None, None], None, 0)
+            kv_bias = b[C:].float().contiguous()
+            self._derived = (sig, q, kv, kv_bias, _linear_conv(enc.attn.out_proj), _linear_conv(enc.linear1),
+                             _linear_conv(enc.linear2))
+        return self._derived[1:]
+
+    def forward_nhwc(self, x, record_len, affine_matrix):
+        """x: Act (sumN,H,W,C) -> Act (B,H,W,C).  Reads record_len on the host; no other sync."""
+        require_eval(self)
+        self._check(x.C)
+        rl = _rl(record_len)
+        if sum(rl) != x.N:
+            raise ValueError(f"Where2commFusion: record_len {rl} does not sum to the {x.N} feature maps")
+        q_conv, kv_conv, kv_bias, out_proj, l1, l2 = self._packed()
+        enc = self.mha_fusion
+        fmt = engine.act_fmt()
+        aff = affine_matrix.to(device=x.device, dtype=torch.float64)
+        starts = [sum(rl[:b]) for b in range(len(rl))]
+        ego = ops.warp_affine(x, starts, aff[:, 0, 0].contiguous(), out_fmt=fmt)
+        theta = torch.cat([aff[b, 0, :n] for b, n in enumerate(rl)])
+        a = ops.ego_mha(conv_bn_act(ego, q_conv), conv_bn_act(x, kv_conv), kv_bias, theta, rl, out_fmt=fmt)
+        y = conv_bn_act(a, out_proj, residual=ego)
+        y1 = ops.mean_layernorm(y, 1, enc.norm1.weight, enc.norm1.bias, enc.norm1.eps, out_fmt=fmt)
+        y = conv_bn_act(conv_bn_act(y1, l1, relu=True), l2, residual=y1)
+        return ops.mean_layernorm(y, 1, enc.norm2.weight, enc.norm2.bias, enc.norm2.eps, out_fmt=fmt)
+
+    def forward(self, x, record_len, affine_matrix):
+        require_eval(self)
+        self._check(x.shape[1])
+        return ops.act_to_nchw(self.forward_nhwc(ops.to_act(x), record_len, affine_matrix))
+
+
+class Who2comFusion(nn.Module):
+    """Who2com's fusion (fusion_in_one.py:486-539) with the reference's ctor and state-dict keys (`decode_layer.*`).
+
+    Per scene, a = the ego row of the parameter-free ScaledDotProductAttention(C) over the agents warped to the ego (exactly
+    AttFusion, heal_att_fuse), then decode_layer(cat[x_0, a]) with x_0 the UNWARPED ego map: heal_att_fuse writes channels
+    [C, 2C) of a (B,H,W,2C) map, the ego is converted into [0, C), and the 3x3 conv runs on the conv engine."""
+
+    def __init__(self, feature_dims):
+        super().__init__()
+        self.att = ScaledDotProductAttention(feature_dims)
+        self.decode_layer = nn.Conv2d(feature_dims * 2, feature_dims, kernel_size=3, stride=1, padding=1)
+        self.feature_dims = feature_dims
+
+    def forward_nhwc(self, x, record_len, affine_matrix):
+        """x: Act (sumN,H,W,C) -> Act (B,H,W,C).  Reads record_len on the host; no other sync."""
+        require_eval(self)
+        C = x.C
+        if C != self.feature_dims:
+            raise ValueError(f"Who2comFusion: feature_dims is {self.feature_dims} but the feature map has {C} channels")
+        rl = _rl(record_len)
+        if sum(rl) != x.N:
+            raise ValueError(f"Who2comFusion: record_len {rl} does not sum to the {x.N} feature maps")
+        fmt = engine.act_fmt()
+        aff = affine_matrix.to(device=x.device, dtype=torch.float64)
+        cat = ops.act_empty(len(rl), x.H, x.W, 2 * C, fmt, x.device)
+        ego, att = ops.Act(cat.t[..., :C], fmt), ops.Act(cat.t[..., C:], fmt)
+        start = 0
+        for b, n in enumerate(rl):
+            ops.att_fuse(x.images(start, start + n), aff[b, 0, :n].contiguous(), out=att.image(b))
+            ops.convert(x.image(start), fmt, out=ego.image(b))
+            start += n
+        return conv_bn_act(cat, self.decode_layer)
+
+    def forward(self, x, record_len, affine_matrix):
         return ops.act_to_nchw(self.forward_nhwc(ops.to_act(x), record_len, affine_matrix))
 
 

@@ -1,7 +1,7 @@
 """HeterModelBaseline mirror (opencood/models/heter_model_baseline.py:26-236): per-modality encoder ->
 BaseBEVBackbone -> per-agent shrinker -> single-scale fusion -> heads.  Same ctor argument, state-dict keys and forward(data_dict) -> output_dict contract.
-`fusion_method`: att (AttFusion), max (F-Cooper MaxFusion), v2vnet (V2VNetFusion), v2xvit (V2XViTFusion) and cobevt (CoBEVT).
-disconet cannot be constructed in the reference itself; where2comm and who2com are outside the hot-path scope."""
+`fusion_method`: att (AttFusion), max (F-Cooper MaxFusion), v2vnet (V2VNetFusion), v2xvit (V2XViTFusion), cobevt (CoBEVT),
+where2comm (Where2commFusion) and who2com (Who2comFusion).  disconet cannot be constructed in the reference itself."""
 import importlib
 from collections import OrderedDict, Counter
 
@@ -13,8 +13,11 @@ from ..engine import require_eval
 from ..utils.transformation_utils import normalize_pairwise_tfm
 from .sub_modules.base_bev_backbone import BaseBEVBackbone
 from .sub_modules.downsample_conv import DownsampleConv
-from .fuse_modules.fusion_in_one import AttFusion, CoBEVT, MaxFusion, V2VNetFusion, V2XViTFusion
+from .fuse_modules.fusion_in_one import (AttFusion, CoBEVT, MaxFusion, V2VNetFusion, V2XViTFusion, Where2commFusion,
+                                         Who2comFusion)
 from .heter_pyramid_collab import FusedHeads, HeterPyramidCollab
+
+_BUILT = "att, max, v2vnet, v2xvit, cobevt, where2comm, who2com"
 
 
 class HeterModelBaseline(nn.Module):
@@ -65,11 +68,20 @@ class HeterModelBaseline(nn.Module):
                 raise NotImplementedError("fusion_method 'v2xvit' without a `v2xvit:` block is outside the heal_b200 hot-path "
                                           "scope (no shipped config omits it)")
             self.fusion_net = V2XViTFusion(args['v2xvit'])
+        elif fm in ("where2comm", "who2com"):
+            if fm not in args:
+                raise NotImplementedError(f"fusion_method '{fm}' without a `{fm}:` block is outside the heal_b200 hot-path "
+                                          f"scope (built: {_BUILT})")
+            dims = args[fm]
+            if not isinstance(dims, int) or isinstance(dims, bool) or dims != 256:
+                raise NotImplementedError(f"fusion_method '{fm}' with `{fm}: {dims!r}` is outside the heal_b200 hot-path "
+                                          "scope (built: the int 256, every baseline yaml's in_head)")
+            self.fusion_net = Where2commFusion(dims) if fm == "where2comm" else Who2comFusion(dims)
         elif fm == "disconet":
             raise NotImplementedError("fusion_method 'disconet': DiscoFusion cannot be constructed in the reference either "
                                       "(it imports opencood.models.fuse_modules.disco_fuse, which the reference does not ship)")
         else:
-            raise NotImplementedError(f"fusion_method '{fm}' is outside the heal_b200 hot-path scope (built: att, max, v2vnet, v2xvit, cobevt)")
+            raise NotImplementedError(f"fusion_method '{fm}' is outside the heal_b200 hot-path scope (built: {_BUILT})")
         self.shrink_flag = 'shrink_header' in args
         if self.shrink_flag:
             self.shrink_conv = DownsampleConv(args['shrink_header'])

@@ -236,10 +236,13 @@ def _theta64(theta: torch.Tensor, n: int) -> torch.Tensor:
 
 
 @_guard
-def convert(a: Act, fmt: str) -> Act:
-    if a.fmt == fmt:
+def convert(a: Act, fmt: str, out: Optional[Act] = None) -> Act:
+    """`a` in storage format `fmt`: `a` itself when it already is, unless `out` (a (N,H,W,C) Act in `fmt`, a channel view of a
+    wider map is fine) is given to receive the copy."""
+    if out is None and a.fmt == fmt:
         return a
-    out = act_empty(a.N, a.H, a.W, a.C, fmt, a.device)
+    out = _out_act(out, a.N, a.H, a.W, a.C, fmt, a.device)
+    assert out.fmt == fmt
     with _Prof("act_convert", 0, a.N * a.H * a.W * float(a.C) * (BPE[a.fmt] + BPE[fmt])):
         _call("heal_act_convert", a.view(), out.view(), a.N * a.H * a.W, a.C)
     return out
@@ -816,6 +819,27 @@ def gru_gate(zc: Act, out: Optional[Act] = None, out_fmt: Optional[str] = None) 
     npix = N * H * W
     with _Prof("gru_gate", 4.0 * npix * C, npix * float(C) * (2 * BPE[zc.fmt] + BPE[out.fmt])):
         _call("heal_gru_gate", zc.view(), npix, C, out.view())
+    return out
+
+
+@_guard
+def ego_mha(q: Act, kv: Act, kv_bias: torch.Tensor, theta: torch.Tensor, n_agents: Sequence[int], heads: int = 8,
+            kv_coffset: int = 0, out: Optional[Act] = None, out_fmt: Optional[str] = None) -> Act:
+    """Where2comm's per-pixel multi-head attention of each scene's warped ego over its warped agents.  q Act (B,H,W,C) = the
+    in-projected warped egos (bias included, unscaled); kv Act (N,H,W,>=kv_coffset+2C) = the bias-free k | v projection of the
+    UNWARPED agent maps from channel kv_coffset, N = sum(n_agents), record_len order; kv_bias (2C) fp32 device; theta (N,2,3)
+    = affine[b, 0, j] stacked scene by scene -> Act (B,H,W,C), the merged heads before out_proj."""
+    _need_cuda(kv_bias, theta)
+    B, H, W, C = len(n_agents), q.H, q.W, q.C
+    N = sum(int(v) for v in n_agents)
+    assert q.N == B and kv.N == N and (kv.H, kv.W) == (H, W) and kv_coffset + 2 * C <= kv.C
+    assert kv_bias.dtype == torch.float32 and kv_bias.is_contiguous() and kv_bias.shape == (2 * C,)
+    th = _theta64(theta, N)
+    out = _out_act(out, B, H, W, C, out_fmt or q.fmt, q.device)
+    with _Prof("ego_mha", 4.0 * N * H * W * C + 16.0 * N * H * W * C,
+               B * H * W * float(C) * (BPE[q.fmt] + BPE[out.fmt]) + N * H * W * 2.0 * C * BPE[kv.fmt]):
+        _call("heal_ego_mha", q.view(), kv.view(kv_coffset), _p(kv_bias), _p(th), _host_i32(n_agents), B, H, W, C, int(heads),
+              out.view())
     return out
 
 

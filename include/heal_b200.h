@@ -214,6 +214,23 @@ int heal_v2v_aggregate(const heal_act_t* q, const heal_act_t* p_node, const heal
                        const int* nodes_host, int n_nodes, int H, int W, int C, int agg_max, int gru,
                        const heal_act_t* out, void* stream);
 
+/* Where2commFusion's attention core (fusion_in_one.py:431-484; where2comm_attn.py EncodeLayer.attn, an 8-head
+ * nn.MultiheadAttention): per scene b, pixel and head, one query (the warped ego) over the scene's n_b agents warped to it.
+ *   q    (B, H, W, C): the in-projected warped ego, bias included, not yet scaled
+ *   kv   (sum n_b, H, W, 2C): [W_k; W_v] x_j of the UNWARPED agent maps, bias-free, in record_len order (each scene's ego
+ *        first); a channel view of a wider map is fine
+ *   kv_bias: (2C) fp32 device, 16-byte aligned: [b_k; b_v], added after sampling
+ *   theta (sum n_b, 2, 3) fp64 device: affine[b, 0, j] stacked scene by scene
+ *   out  (B, H, W, C): the merged heads, before out_proj
+ * k_j = warp(kv_j, theta_j)[:C] + b_k and v_j = warp(kv_j, theta_j)[C:] + b_v (bilinear, zeros padding, align_corners=False:
+ * the taps of heal_att_fuse; a linear map commutes with the warp, so this is the projection of the warped map).  Per head:
+ * out = sum_j softmax_j((q * dim_head^-0.5) . k_j) v_j, the scale applied to q in fp32 as PyTorch does, the max subtracted
+ * before the exponent, agents summed in order; fp32 math for every storage format, no atomics (bit-identical reruns).
+ * C = 256 and heads = 8 (dim_head 32), else HEAL_ERR_UNSUPPORTED.  n_agents_host: HOST array of B counts in [1, 8], all checked
+ * before anything is launched (else HEAL_ERR_ARG).  Alignment of q, kv and out as heal_max_fuse. */
+int heal_ego_mha(const heal_act_t* q, const heal_act_t* kv, const float* kv_bias, const double* theta,
+                 const int* n_agents_host, int B, int H, int W, int C, int heads, const heal_act_t* out, void* stream);
+
 /* ConvGRU cell with a zero hidden state (sub_modules/convgru.py:47-68): out(npix,C) = sigmoid(zc[:, :C]) * tanh(zc[:, C:2C]),
  * zc = the stacked (update gate | candidate) GRU conv output (npix, 2C).  Alignment of zc and out as heal_max_fuse. */
 int heal_gru_gate(const heal_act_t* zc, long long npix, int C, const heal_act_t* out, void* stream);
