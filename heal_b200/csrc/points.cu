@@ -23,7 +23,7 @@ __global__ void k_mask_flags(MaskP p, int* __restrict__ flags) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= p.P) return;
     int keep = 0;
-    if (i < p.offs[p.A]) {
+    if (i >= p.offs[0] && i < p.offs[p.A]) {         // rows before offs[0] belong to no agent: the output offsets start at 0
         const float4 q = src_point(p, i);
         keep = (q.x > p.lo[0]) && (q.x < p.hi[0]) && (q.y > p.lo[1]) && (q.y < p.hi[1]) && (q.z > p.lo[2]) && (q.z < p.hi[2]);
         if (p.remove_ego && (q.x >= -1.95f) && (q.x <= 2.95f) && (q.y >= -1.1f) && (q.y <= 1.1f)) keep = 0;

@@ -13,6 +13,8 @@
 //   3. per-agent clamp to max_voxels, output base per agent, voxel id per cell       [k_agent_bases, k_assign]
 //   4. per-voxel point count -> scan -> CSR fill (unordered)                         [k_count, scan, k_fill]
 //   5. one warp per voxel selects the T smallest point indices in ascending order    [k_select]
+// Agent a owns rows [offs[a], offs[a+1]); rows outside [offs[0], offs[A]) are ignored.  Voxel rows at or past `capacity` are
+// dropped (not written, their points not counted), while num_voxels_out keeps the true counts.
 // Every step is deterministic in its OUTPUT (atomics only build unordered sets that are ordered
 // afterwards), so indices/counts/features are bit-exact with the CPU generator.
 #include "common.cuh"
@@ -43,8 +45,9 @@ __global__ void k_cells_insert(const float4* __restrict__ pts, const int* __rest
                                uint32_t* __restrict__ keys, int* __restrict__ firsts, int* __restrict__ pt_slot) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= c.P) return;
-    // `P` may be the CAPACITY of a static (CUDA-graph) input buffer: the live point count is offs[A] on the device
-    if (i >= offs[c.A]) { pt_slot[i] = -1; return; }
+    // `P` may be the CAPACITY of a static (CUDA-graph) input buffer: the live point count is offs[A] on the device.
+    // Rows before offs[0] belong to no agent.
+    if (i < offs[0] || i >= offs[c.A]) { pt_slot[i] = -1; return; }
     float4 p = __ldg(pts + i);
     // IEEE fp32 subtract + divide + floor, exactly as the CPU generator (no reciprocal multiply).
     float fx = floorf(__fdiv_rn(__fsub_rn(p.x, c.minx), c.vsx));
@@ -155,6 +158,7 @@ __global__ void k_assign(const int* __restrict__ offs, const int* __restrict__ p
     int rank = local_excl[i] + block_off[i / SCAN_BLOCK];
     int local = rank - meta[a];
     int vid = (local < c.maxV) ? (meta[c.A + 1 + a] + local) : -1;
+    if (vid >= c.cap) vid = -1;   // rows past the output capacity are dropped; num_voxels_out still counts them
     slot_vid[s] = vid;
     if (vid >= 0) {
         uint32_t cell = keys[s] - (uint32_t)a * c.cells;
@@ -189,12 +193,12 @@ __global__ void k_fill(const int* __restrict__ pt_vid, int P, const int* __restr
 // zero-padded (T,4) feature block and the point count.
 __global__ void k_select(const float4* __restrict__ pts, const int* __restrict__ seg, const int* __restrict__ cnt,
                          const int* __restrict__ seg_local, const int* __restrict__ seg_blockoff,
-                         const int* __restrict__ num_voxels, int T,
+                         const int* __restrict__ num_voxels, int T, int cap,
                          float4* __restrict__ voxels, int* __restrict__ num_points) {
     // persistent warps: the launch is sized for the machine, not for the row CAPACITY (the live voxel count is on the device
     // and typically 4-5x below the capacity: a capacity-sized grid spent most of its blocks on an early exit)
     const int lane = threadIdx.x & 31;
-    const int nv = num_voxels[0];
+    const int nv = min(num_voxels[0], cap);
     const int wstride = (gridDim.x * blockDim.x) >> 5;
     for (int v = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; v < nv; v += wstride) {
     int n = cnt[v];
@@ -328,7 +332,7 @@ extern "C" int heal_voxelize(const float* points, const int* agent_offsets, int 
     int gv = (int)(((size_t)capacity * 32 + TB - 1) / TB);
     if (gv > HEAL_NUM_SMS * 8) gv = HEAL_NUM_SMS * 8;           // 8 resident blocks of 8 warps per SM, warp-stride loop over the voxels
     k_select<<<gv, TB, 0, st>>>((const float4*)points, seg, cnt, seg_local, seg_blockoff, num_voxels_out,
-                                c.T, (float4*)voxels_out, num_points_out);
+                                c.T, capacity, (float4*)voxels_out, num_points_out);
     return heal_check_launch(10);
 }
 

@@ -52,11 +52,13 @@ long long heal_launch_count(void);
  * first appearance, first `max_points_per_voxel` points in input order, cells beyond `max_voxels`
  * dropped, coords = [agent, z, y, x].
  *   points          (P_total,4) f32, agents concatenated
- *   agent_offsets   (A+1) i32 device: points of agent a are [off[a], off[a+1])
+ *   agent_offsets   (A+1) i32 device: points of agent a are [off[a], off[a+1]); rows before off[0] and from off[A] on
+ *                   are ignored
  *   range_min3/voxel_size3/grid3   HOST arrays (x,y,z)
- *   capacity        rows available in the outputs (>= number of voxels produced)
+ *   capacity        rows available in the outputs; voxel rows >= capacity are dropped (nothing is written past it)
  *   voxels_out      (capacity,T,4) f32   coords_out (capacity,4) i32   num_points_out (capacity) i32
- *   num_voxels_out  (1+A) i32: [0] = M total, [1+a] = voxels of agent a */
+ *   num_voxels_out  (1+A) i32: [0] = M total, [1+a] = voxels of agent a, counted before the capacity cut, so
+ *                   min(M, capacity) rows are valid */
 size_t heal_voxelize_workspace(int num_points_total, int capacity, int num_agents);
 int heal_voxelize(const float* points, const int* agent_offsets, int num_agents, int num_points_total,
                   const float* range_min3_host, const float* voxel_size3_host, const int* grid3_host,
@@ -515,7 +517,8 @@ int heal_p2p_signal_wait(void* const* peer_flags_host, int world, int self, unsi
  * shuffle_points / mask_ego_points / mask_points_by_range (opencood/utils/pcd_utils.py:41-95, applied in this order by
  * intermediate_heter_fusion_dataset.py:141-173) as one stable compaction per agent: points_out = mask(points[perm]).
  *   points (P,4) f32, agents concatenated; perm (P) i32 GLOBAL source index per slot (the host-drawn shuffle) or NULL;
- *   agent_offsets (A+1) i32 device (live count = offsets[A] <= P); range6_host = [xmin,ymin,zmin,xmax,ymax,zmax] (strict);
+ *   agent_offsets (A+1) i32 device (live count = offsets[A] <= P; rows before offsets[0] are dropped, so
+ *   agent_offsets_out[0] = 0); range6_host = [xmin,ymin,zmin,xmax,ymax,zmax] (strict);
  *   remove_ego != 0 drops the ego-vehicle box.  points_out (P,4); agent_offsets_out (A+1) i32 device. */
 size_t heal_mask_points_workspace(int num_points);
 int heal_mask_points(const float* points, const int* perm, const int* agent_offsets, int num_agents, int num_points,
