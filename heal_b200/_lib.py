@@ -41,6 +41,7 @@ SIGNATURES = {
                               _i, _i, _i, _i, _vp]),
     "heal_conv2d_tc": (_i, [_vp, _sz, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _i,
                             _vp, _sz, _vp, _i, _i, _vp, _sz, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "heal_conv3x3_narrow_tc": (_i, [_ap, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _ap, _vp]),
     "heal_bottleneck_tc": (_i, [_vp, _sz, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _sz, _i, _i, _vp]),
     "heal_dwconv_layernorm": (_i, [_ap, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _c.c_float, _ap, _vp]),
     "heal_maxpool3x3s2": (_i, [_ap, _i, _i, _i, _i, _i, _ap, _vp]),

@@ -67,6 +67,12 @@ def packed(conv: nn.Module, bn: Optional[nn.Module], relu: bool, extra_pad: int 
         return hit[1]
     if kind == "simt":
         pc = ops.pack_deconv(conv, bn, relu) if isinstance(conv, nn.ConvTranspose2d) else ops.pack_conv(conv, bn, relu, extra_pad)
+    elif kind == "simt_cin4":
+        pc = ops.pack_conv(conv, bn, relu, extra_pad, cin_to=(conv.in_channels + 3) // 4 * 4)
+    elif kind == "narrow":
+        pc = ops.pack_conv3x3_narrow(conv, bn, relu)
+    elif kind == "tc2_cin64":
+        pc = ops.pack_conv_tc(conv, bn, relu, planes=2, extra_pad=extra_pad, cin_to=(conv.in_channels + 63) // 64 * 64)
     else:
         pc = ops.pack_conv_tc(conv, bn, relu, planes=2 if kind == "tc2" else 1, extra_pad=extra_pad)
     pc.to(conv.weight.device)

@@ -22,6 +22,7 @@ _MAP = {
     "opencood.models.sub_modules.base_bev_backbone_resnet": "heal_b200.models.sub_modules.base_bev_backbone_resnet",
     "opencood.models.sub_modules.resblock": "heal_b200.models.sub_modules.resblock",
     "opencood.models.sub_modules.downsample_conv": "heal_b200.models.sub_modules.downsample_conv",
+    "opencood.models.sub_modules.naive_compress": "heal_b200.models.sub_modules.naive_compress",
 }
 
 

@@ -13,6 +13,7 @@ from ..engine import require_eval
 from ..utils.transformation_utils import normalize_pairwise_tfm
 from .sub_modules.base_bev_backbone import BaseBEVBackbone
 from .sub_modules.downsample_conv import DownsampleConv
+from .sub_modules.naive_compress import NaiveCompressor
 from .fuse_modules.fusion_in_one import (AttFusion, CoBEVT, MaxFusion, V2VNetFusion, V2XViTFusion, Where2commFusion,
                                          Who2comFusion)
 from .heter_pyramid_collab import FusedHeads, HeterPyramidCollab
@@ -88,13 +89,13 @@ class HeterModelBaseline(nn.Module):
         self.cls_head = nn.Conv2d(args['in_head'], args['anchor_number'], kernel_size=1)
         self.reg_head = nn.Conv2d(args['in_head'], 7 * args['anchor_number'], kernel_size=1)
         self.dir_head = nn.Conv2d(args['in_head'], args['dir_args']['num_bins'] * args['anchor_number'], kernel_size=1)
-        if 'compressor' in args:
-            raise NotImplementedError("NaiveCompressor is training-time only in HEAL and not on the inference hot path")
-        self.compress = False
+        self.compress = 'compressor' in args
+        if self.compress:
+            self.compressor = NaiveCompressor(args['compressor']['input_dim'], args['compressor']['compress_ratio'])
         self._heads = FusedHeads([self.cls_head, self.reg_head, self.dir_head])
+        self.model_train_init()
 
-    def model_train_init(self):
-        pass
+    model_train_init = HeterPyramidCollab.model_train_init
 
     def forward(self, data_dict):
         require_eval(self)
@@ -127,6 +128,8 @@ class HeterModelBaseline(nn.Module):
                 rows.append(ops.convert(feats[m].image(cnt[m]), "f32").t)
                 cnt[m] += 1
             x = ops.Act(torch.cat(rows, 0), "f32")
+        if self.compress:
+            x = self.compressor.forward_nhwc(x)
         if self.supervise_single:
             c, r, d = self._heads_single(x)
             output_dict.update({'cls_preds_single': c, 'reg_preds_single': r, 'dir_preds_single': d})

@@ -12,6 +12,7 @@ from ..utils.transformation_utils import normalize_pairwise_tfm
 from .sub_modules.base_bev_backbone_resnet import ResNetBEVBackbone
 from .sub_modules.feature_alignnet import AlignNet
 from .sub_modules.downsample_conv import DownsampleConv
+from .sub_modules.naive_compress import NaiveCompressor
 from .fuse_modules.pyramid_fuse import PyramidFusion
 
 
@@ -91,11 +92,20 @@ class HeterPyramidCollab(nn.Module):
         self.dir_head = nn.Conv2d(args['in_head'], args['dir_args']['num_bins'] * args['anchor_number'], kernel_size=1)
         self.compress = 'compressor' in args
         if self.compress:
-            raise NotImplementedError("NaiveCompressor is training-time only in HEAL and not on the inference hot path")
+            self.compressor = NaiveCompressor(args['compressor']['input_dim'], args['compressor']['compress_ratio'])
         self._heads = FusedHeads([self.cls_head, self.reg_head, self.dir_head])
+        self.model_train_init()
 
     def model_train_init(self):
-        pass
+        """The reference's: with a compressor, freeze everything and leave only the compressor in train mode (the forward then
+        refuses to run until `.eval()`: training is not implemented)."""
+        if self.compress:
+            self.eval()
+            for p in self.parameters():
+                p.requires_grad_(False)
+            self.compressor.train()
+            for p in self.compressor.parameters():
+                p.requires_grad_(True)
 
     @staticmethod
     def _center_crop_nhwc(act, th, tw):
@@ -149,6 +159,8 @@ class HeterPyramidCollab(nn.Module):
                 rows.append(ops.convert(feats[m].image(cnt[m]), "f32").t)
                 cnt[m] += 1
             x = ops.Act(torch.cat(rows, 0), "f32")
+        if self.compress:
+            x = self.compressor.forward_nhwc(x)
         fused, occs = self.pyramid_backbone.forward_collab_nhwc(x, record_len, affine, aml, self.cam_crop_info)
         if self.shrink_flag:
             fused = self.shrink_conv.forward_nhwc(fused)

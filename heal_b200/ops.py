@@ -453,11 +453,17 @@ class PackedConv:
         return self
 
 
-def pack_conv(conv: torch.nn.Conv2d, bn: Optional[torch.nn.Module], relu: bool, extra_pad: int = 0) -> PackedConv:
-    """Fold eval-mode BN into the conv (fp64 on the host) and pack for heal_conv2d_simt."""
+def pack_conv(conv: torch.nn.Conv2d, bn: Optional[torch.nn.Module], relu: bool, extra_pad: int = 0,
+              cin_to: Optional[int] = None) -> PackedConv:
+    """Fold eval-mode BN into the conv (fp64 on the host) and pack for heal_conv2d_simt.  `cin_to` (groups 1): zero weights for
+    input channels [Cin, cin_to), for an input whose channel count is padded to the multiple of 4 the kernel reads."""
     w = conv.weight.detach().double().cpu()            # (Cout, Cin/g, kh, kw)
     cout, cing, kh, kw = w.shape
     g = conv.groups
+    if cin_to is not None and cin_to > cing:
+        assert g == 1
+        w = torch.cat([w, w.new_zeros((cout, cin_to - cing, kh, kw))], 1)
+        cing = cin_to
     scale, shift = _bn_scale_shift(bn, cout)
     b = shift.clone()
     if conv.bias is not None:
@@ -536,8 +542,9 @@ def tc_eligible(conv) -> bool:
     return TC_GROUPED and conv.in_channels == conv.out_channels and conv.kernel_size == (3, 3) and 16 % cg == 0
 
 
-def pack_conv_tc(conv, bn, relu: bool, planes: int = 2, extra_pad: int = 0) -> PackedConvTC:
-    """Fold BN (fp64), lay weights out as [plane][tap*coutp + co][Cin] (split-)bf16 for heal_conv2d_tc."""
+def pack_conv_tc(conv, bn, relu: bool, planes: int = 2, extra_pad: int = 0, cin_to: Optional[int] = None) -> PackedConvTC:
+    """Fold BN (fp64), lay weights out as [plane][tap*coutp + co][Cin] (split-)bf16 for heal_conv2d_tc.  `cin_to` (dense convs):
+    zero weights for input channels [Cin, cin_to), for an input zero-padded to a multiple of 64 channels."""
     if isinstance(conv, torch.nn.ConvTranspose2d):
         w = conv.weight.detach().double().cpu()            # (Cin, Cout, k, k)
         cin, cout, k, _ = w.shape
@@ -575,11 +582,55 @@ def pack_conv_tc(conv, bn, relu: bool, planes: int = 2, extra_pad: int = 0) -> P
         pc.w_diag = split_bf16(diag.reshape(kh * kw * width, 16).float(), planes)
         return pc
     coutp = _coutp(cout)
+    cin_w = cin
+    if cin_to is not None and cin_to > cin:
+        cin = cin_to
     rows = torch.zeros((kh * kw, coutp, cin), dtype=torch.float64)
-    rows[:, :cout, :] = w.permute(2, 3, 0, 1).reshape(kh * kw, cout, cin)
+    rows[:, :cout, :cin_w] = w.permute(2, 3, 0, 1).reshape(kh * kw, cout, cin_w)
     wp = split_bf16(rows.reshape(kh * kw * coutp, cin).float(), planes)
     return PackedConvTC(wp, b.float().contiguous(), kh, kw, conv.padding[0] + extra_pad, cin, cout, coutp, relu, 1, planes,
                         stride=conv.stride[0])
+
+
+class PackedConvNarrow:
+    """Folded + packed parameters of one 3x3 Conv2d(+BN)(+ReLU) with a narrow input for heal_conv3x3_narrow_tc."""
+
+    def __init__(self, w, bias, cin, cout, relu):
+        self.w, self.bias, self.cin, self.cout, self.relu = w, bias, cin, cout, relu
+
+    def to(self, device):
+        self.w = self.w.to(device)
+        self.bias = self.bias.to(device)
+        return self
+
+
+def narrow_eligible(conv) -> bool:
+    """A conv heal_conv3x3_narrow_tc takes: 3x3, stride 1, pad 1, groups 1, 1 <= Cin <= 63, Cout a multiple of 16 up to 256."""
+    return (isinstance(conv, torch.nn.Conv2d) and conv.kernel_size == (3, 3) and conv.stride == (1, 1)
+            and conv.padding == (1, 1) and conv.dilation == (1, 1) and conv.groups == 1 and 1 <= conv.in_channels <= 63
+            and conv.out_channels % 16 == 0 and conv.out_channels <= 256)
+
+
+def pack_conv3x3_narrow(conv, bn, relu: bool) -> PackedConvNarrow:
+    """Fold BN (fp64) and lay the weights out as heal_conv3x3_narrow_tc reads them: K = (tap, channel) with the channel count
+    rounded up to even, padded to a multiple of 16; per 64-channel output block and 64-wide K block [hi 64 rows | lo 64 rows]."""
+    assert narrow_eligible(conv)
+    w = conv.weight.detach().double().cpu()                # (Cout, Cin, 3, 3)
+    cout, cin = w.shape[:2]
+    scale, shift = _bn_scale_shift(bn, cout)
+    b = shift + (conv.bias.detach().double().cpu() * scale if conv.bias is not None else 0)
+    w = w * scale[:, None, None, None]
+    cinp = cin + (cin & 1)
+    k = (9 * cinp + 15) // 16 * 16
+    kb, nblk = (k + 63) // 64, (cout + 63) // 64
+    rows = torch.zeros((nblk * 64, 9, cinp), dtype=torch.float64)
+    rows[:cout, :, :cin] = w.permute(0, 2, 3, 1).reshape(cout, 9, cin)
+    mat = torch.zeros((nblk * 64, kb * 64), dtype=torch.float32)
+    mat[:, :9 * cinp] = rows.reshape(nblk * 64, 9 * cinp).float()
+    hi, lo = split_bf16(mat, 2)                            # (nblk*64, kb*64) each
+    wp = torch.stack([hi.view(nblk, 64, kb, 64), lo.view(nblk, 64, kb, 64)], 2)   # (nblk, 64 rows, plane, kb, 64)
+    wp = wp.permute(0, 3, 2, 1, 4).contiguous()            # (nblk, kb, plane, 64 rows, 64)
+    return PackedConvNarrow(wp, b.float().contiguous(), cin, cout, relu)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -656,6 +707,22 @@ def conv2d_tc(x: Act, pc: PackedConvTC, residual: Optional[Act] = None, out: Opt
               out_f32.cstride if out_f32 is not None else 0, out32_coffset,
               Ho, Wo, pc.cout, up, int(pc.relu))
     return out, out_f32
+
+
+@_guard
+def conv3x3_narrow_tc(x: Act, pc: PackedConvNarrow, planes: int, out: Optional[Act] = None, out_fmt: str = "split") -> Act:
+    """wgmma 3x3 conv of a narrow input (Cin < 64).  x: any storage format, may be a channel slice of a wider map.  planes 2:
+    split-bf16 products ('tc32'), 1: bf16 activations x split weights ('bf16').  `out` (optional): (N,H,W,Cout) Act."""
+    _need_cuda(pc.w)
+    assert x.C == pc.cin and planes in (1, 2)
+    N, H, W = x.N, x.H, x.W
+    out = _out_act(out, N, H, W, pc.cout, out_fmt, x.device)
+    flops = 2.0 * N * H * W * pc.cout * pc.cin * 9
+    nbytes = N * H * W * (pc.cin * BPE[x.fmt] + pc.cout * BPE[out.fmt]) + pc.w.numel() * 2.0
+    with _Prof("conv_tc3x3_narrow", flops, nbytes):
+        _call("heal_conv3x3_narrow_tc", x.view(), N, H, W, pc.cin, _p(pc.w), _p(pc.bias), pc.cout, planes, int(pc.relu),
+              out.view())
+    return out
 
 
 @_guard

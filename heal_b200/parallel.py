@@ -82,9 +82,16 @@ def all_gather_bytes(local: torch.Tensor, world: int) -> torch.Tensor:
     return out
 
 
+def _refuse_compressor(model):
+    if getattr(model, "compress", False):
+        raise NotImplementedError(f"{type(model).__name__} with a `compressor:`: the agent-sharded path does not apply the "
+                                  "compressor; run the model on one GPU")
+
+
 def forward_agent_sharded(model, data_dict, rank: int, world: int):
     """HeterPyramidCollab.forward with the per-agent part sharded over `world` ranks (single lidar modality 'm1').
     data_dict carries the WHOLE scene on every rank (raw points + agent_offsets); each rank touches only its agents' points."""
+    _refuse_compressor(model)
     from . import ops
     from .engine import act_fmt
     from .utils.transformation_utils import normalize_pairwise_tfm
@@ -282,6 +289,7 @@ class AgentShardedFrame:
 
     def __init__(self, model, n_agents: int, rank: int, world: int, point_capacity: int, pairwise_shape, device=None,
                  modality: str = "m1", shard_tail: bool = True, group=None, warmup: int = 2, comm: str = "auto"):
+        _refuse_compressor(model)
         from . import ops
         from .engine import act_fmt
         from ._lib import lib

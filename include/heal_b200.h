@@ -150,6 +150,24 @@ int heal_conv2d_tc(const void* in_split, size_t in_plane_stride, int N, int H, i
                    float* out_f32, int out32_cstride, int out32_coffset,
                    int Ho, int Wo, int Cout, int upsample, int relu, void* stream);
 
+/* ---- 3x3 convolution of a narrow input, wgmma tensor-core path -----------------------------------
+ * out = act(conv3x3(in) + bias), stride 1, pad 1, groups 1, for 1 <= Cin <= 63 (NaiveCompressor's first decoder conv: the
+ * compressed map is narrower than heal_conv2d_tc's 64-channel K blocks).  The implicit GEMM's K is the whole neighbourhood:
+ * k = tap * cinp + ci with tap = ky * 3 + kx, cinp = Cin rounded up to even, K = 9 * cinp rounded up to a multiple of 16.
+ *   in         any storage format (f32, bf16, split), any channel stride >= coffset + Cin (a channel slice is fine)
+ *   w_packed   bf16 [ceil(Cout / 64)][ceil(K / 64)][128][64], 16-byte aligned: per 64-channel output block and 64-wide K block,
+ *              rows 0..63 = hi = bf16(w) and rows 64..127 = lo = bf16(w - hi) of output channels 64 * block + row, column = k;
+ *              zero in the pad channel of an odd Cin, for k >= 9 * cinp and for channels >= Cout; BN scale folded
+ *   bias       fp32 [Cout] (folded BN shift), 8-byte aligned
+ *   planes     2: split-bf16 activations, a_hi*b_lo + a_lo*b_hi + a_hi*b_hi per K step (fp32-equivalent, "tc32");
+ *              1: bf16 activations, a_hi*b_lo + a_hi*b_hi ("bf16").  The input is read as fp32 and split by the kernel.
+ *   relu       0 | 1
+ *   out        (N,H,W,Cout) in any storage format; channel stride, offset and plane stride even, data 8-byte (f32) or
+ *              4-byte (bf16, split) aligned, else HEAL_ERR_UNSUPPORTED.
+ * Cout is a multiple of 16 in [16, 256].  Allocates nothing and does not synchronise. */
+int heal_conv3x3_narrow_tc(const heal_act_t* in, int N, int H, int W, int Cin, const void* w_packed, const float* bias,
+                           int Cout, int planes, int relu, const heal_act_t* out, void* stream);
+
 /* ---- ResNeXt bottleneck, fused (PyramidFusion level 0) ------------------------------------------
  * y = ReLU(conv3(ReLU(conv2(ReLU(conv1(x))))) + x) for the stride-1 Bottleneck with C = 64 input / output channels, width 128,
  * 32 groups and no downsample (BN folded into each conv), as one kernel: the width-128 intermediates stay on chip.  The three
