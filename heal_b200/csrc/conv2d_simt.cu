@@ -22,6 +22,7 @@ struct ConvP {
     int relu;
     int up, up_i, up_j;                      // output pixel (oh,ow) is stored at (oh*up+up_i, ow*up+up_j) of an (Ho*up, Wo*up) map
     int groups;
+    int out_vec4;                            // the output view takes act_store4 (aligned4 on the host)
 };
 
 constexpr int BM = 128, BN = 64, BK = 16;
@@ -123,7 +124,7 @@ k_conv2d_dense(ConvP p) {
 #pragma unroll
             for (int j = 0; j < 4; ++j) v[j] = heal_act_fn(v[j], p.relu);
         }
-        if (co + 3 < p.Cout && ((p.out.cs | p.out.co) & 3) == 0) {
+        if (co + 3 < p.Cout && p.out_vec4) {
             act_store4(p.out, pix, co, make_float4(v[0], v[1], v[2], v[3]));
         } else {
 #pragma unroll
@@ -238,6 +239,14 @@ static inline ActV to_view(const heal_act_t* a) {
     return v;
 }
 
+// act_load4 / act_store4 move 4 channels at once: every 4-channel group starts 16 B-aligned in fp32 and 8 B-aligned in each bf16
+// plane, so the base pointer as well as the channel stride, offset and (split) plane stride.
+static inline bool aligned4(const heal_act_t* a) {
+    const uintptr_t need = a->fmt == 0 ? 15 : 7;
+    return ((uintptr_t)a->data & need) == 0 && (a->cstride & 3) == 0 && (a->coffset & 3) == 0 &&
+           (a->fmt != 2 || (a->plane_stride & 3) == 0);
+}
+
 extern "C" int heal_conv2d_simt(const heal_act_t* in, int N, int H, int W, int Cin,
                                 const float* weight, int w_cstride, const float* bias,
                                 int kh, int kw, int stride, int pad, int groups,
@@ -245,15 +254,15 @@ extern "C" int heal_conv2d_simt(const heal_act_t* in, int N, int H, int W, int C
                                 int upsample, int up_i, int up_j, int relu, void* stream_) {
     if (!in || !in->data || !weight || !out || !out->data) return HEAL_ERR_ARG;
     if (N < 1 || H < 1 || W < 1 || Cin < 1 || Cout < 1 || Ho < 1 || Wo < 1 || stride < 1 || upsample < 1) return HEAL_ERR_ARG;
-    if ((in->cstride & 3) || (in->coffset & 3) || (Cin & 3)) return HEAL_ERR_UNSUPPORTED;
     if (in->fmt < 0 || in->fmt > 2 || out->fmt < 0 || out->fmt > 2) return HEAL_ERR_ARG;
+    if (!aligned4(in) || (Cin & 3)) return HEAL_ERR_UNSUPPORTED;
     ConvP p;
     p.in = to_view(in); p.res = to_view(residual); p.out = to_view(out);
     p.w = weight; p.bias = bias;
     p.N = N; p.H = H; p.W = W; p.Cin = Cin;
     p.Ho = Ho; p.Wo = Wo; p.Cout = Cout;
     p.kh = kh; p.kw = kw; p.stride = stride; p.pad = pad; p.w_cs = w_cstride; p.relu = relu;
-    p.up = upsample; p.up_i = up_i; p.up_j = up_j; p.groups = groups;
+    p.up = upsample; p.up_i = up_i; p.up_j = up_j; p.groups = groups; p.out_vec4 = aligned4(out);
     cudaStream_t st = (cudaStream_t)stream_;
     if (groups == 1) {
         if (w_cstride & 3) return HEAL_ERR_UNSUPPORTED;
@@ -264,7 +273,7 @@ extern "C" int heal_conv2d_simt(const heal_act_t* in, int N, int H, int W, int C
     }
     // grouped: 3x3, Cin == Cout, CG = Cin/groups in {4,8,16}, no residual/upsample
     if (kh != 3 || kw != 3 || Cin != Cout || residual || upsample != 1 || (groups % 32) != 0) return HEAL_ERR_UNSUPPORTED;
-    if ((out->cstride & 3) || (out->coffset & 3)) return HEAL_ERR_UNSUPPORTED;
+    if (!aligned4(out)) return HEAL_ERR_UNSUPPORTED;
     int cg = Cin / groups;
     if (cg * groups != Cin) return HEAL_ERR_ARG;
     if (cg == 4) return launch_grouped<4, 4, 4>(p, st);

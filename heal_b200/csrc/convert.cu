@@ -23,10 +23,19 @@ __global__ void k_act_convert_scalar(ActV src, ActV dst, size_t npix, int channe
 }
 }  // namespace
 
+// act_load4 / act_store4 move 4 channels at once: every 4-channel group starts 16 B-aligned in fp32 and 8 B-aligned in each bf16
+// plane, so the base pointer as well as the channel stride, offset and (split) plane stride.
+static inline bool aligned4(const heal_act_t* a) {
+    const uintptr_t need = a->fmt == 0 ? 15 : 7;
+    return ((uintptr_t)a->data & need) == 0 && (a->cstride & 3) == 0 && (a->coffset & 3) == 0 &&
+           (a->fmt != 2 || (a->plane_stride & 3) == 0);
+}
+
 extern "C" int heal_act_convert(const heal_act_t* src, const heal_act_t* dst, size_t num_pixels, int channels, void* stream_) {
-    if (!src || !dst || !src->data || !dst->data) return HEAL_ERR_ARG;
-    if (num_pixels == 0) return HEAL_OK;
-    const bool vec = !((channels & 3) || (src->cstride & 3) || (src->coffset & 3) || (dst->cstride & 3) || (dst->coffset & 3));
+    if (!src || !dst) return HEAL_ERR_ARG;
+    if (num_pixels == 0) return HEAL_OK;            // an empty map may have no storage (a null data pointer)
+    if (!src->data || !dst->data) return HEAL_ERR_ARG;
+    const bool vec = (channels & 3) == 0 && aligned4(src) && aligned4(dst);
     ActV s, d;
     s.p = src->data; s.fmt = src->fmt; s.cs = src->cstride; s.co = src->coffset; s.plane = src->plane_stride;
     d.p = dst->data; d.fmt = dst->fmt; d.cs = dst->cstride; d.co = dst->coffset; d.plane = dst->plane_stride;

@@ -153,6 +153,14 @@ static inline ActV view_of(const heal_act_t* a) {
     return v;
 }
 
+// act_load4 / act_store4 move 4 channels at once: every 4-channel group starts 16 B-aligned in fp32 and 8 B-aligned in each bf16
+// plane, so the base pointer as well as the channel stride, offset and (split) plane stride.
+static inline bool aligned4(const heal_act_t* a) {
+    const uintptr_t need = a->fmt == 0 ? 15 : 7;
+    return ((uintptr_t)a->data & need) == 0 && (a->cstride & 3) == 0 && (a->coffset & 3) == 0 &&
+           (a->fmt != 2 || (a->plane_stride & 3) == 0);
+}
+
 }  // namespace
 
 extern "C" int heal_dwconv_layernorm(const heal_act_t* in, int N, int H, int W, int C, const float* dw_weight, const float* dw_bias,
@@ -160,6 +168,7 @@ extern "C" int heal_dwconv_layernorm(const heal_act_t* in, int N, int H, int W, 
                                      void* stream_) {
     if (!in || !in->data || !out || !out->data || !dw_weight || !ln_weight || !ln_bias) return HEAL_ERR_ARG;
     if ((C % 64) || C > 256 || ksize < 1 || !(ksize & 1) || ksize > 11) return HEAL_ERR_UNSUPPORTED;
+    if ((uintptr_t)dw_weight & 7) return HEAL_ERR_UNSUPPORTED;     // read as float2
     DwLnP p;
     p.in = view_of(in); p.out = view_of(out); p.w = dw_weight; p.b = dw_bias; p.lnw = ln_weight; p.lnb = ln_bias;
     p.N = N; p.H = H; p.W = W; p.C = C; p.k = ksize; p.eps = eps;
@@ -171,7 +180,7 @@ extern "C" int heal_dwconv_layernorm(const heal_act_t* in, int N, int H, int W, 
 extern "C" int heal_maxpool3x3s2(const heal_act_t* in, int N, int H, int W, int C, int depth_to_space_in, const heal_act_t* out, void* stream_) {
     if (!in || !in->data || !out || !out->data) return HEAL_ERR_ARG;
     if (depth_to_space_in && ((H | W) & 1)) return HEAL_ERR_UNSUPPORTED;
-    if ((C & 3) || (in->cstride & 3) || (in->coffset & 3) || (out->cstride & 3) || (out->coffset & 3)) return HEAL_ERR_UNSUPPORTED;
+    if ((C & 3) || !aligned4(in) || !aligned4(out)) return HEAL_ERR_UNSUPPORTED;
     const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
     const long long total = (long long)N * Ho * Wo * (C / 4);
     k_maxpool3s2<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(view_of(in), view_of(out), N, H, W, C, Ho, Wo, depth_to_space_in);
@@ -180,12 +189,13 @@ extern "C" int heal_maxpool3x3s2(const heal_act_t* in, int N, int H, int W, int 
 
 extern "C" int heal_mean_layernorm(const heal_act_t* in, int n_out, int n_avg, int H, int W, int C, const float* ln_weight,
                                    const float* ln_bias, float eps, const heal_act_t* out, void* stream_) {
-    if (!in || !in->data || !out || !out->data || !ln_weight || !ln_bias || n_out < 0 || n_avg < 1 || H < 1 || W < 1) return HEAL_ERR_ARG;
+    if (!in || !out || !ln_weight || !ln_bias || n_out < 0 || n_avg < 1 || H < 1 || W < 1) return HEAL_ERR_ARG;
     if ((C % 64) || C < 64 || C > 256) return HEAL_ERR_UNSUPPORTED;
+    if (n_out == 0) return HEAL_OK;                 // an empty map may have no storage (a null data pointer)
+    if (!in->data || !out->data) return HEAL_ERR_ARG;
     MeanLnP p;
     p.in = view_of(in); p.out = view_of(out); p.lnw = ln_weight; p.lnb = ln_bias;
     p.npix = (long long)n_out * H * W; p.HW = H * W; p.C = C; p.n_avg = n_avg; p.eps = eps;
-    if (p.npix == 0) return HEAL_OK;
     k_mean_layernorm<<<(unsigned)((p.npix + 7) / 8), 256, 0, (cudaStream_t)stream_>>>(p);
     return heal_check_launch();
 }

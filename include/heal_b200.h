@@ -28,7 +28,8 @@ extern "C" {
 
 /* Activation tensor view (channels-last).  fmt: 0 = fp32, 1 = bf16 (one plane), 2 = split-bf16
  * (hi = bf16(x) at data, lo = bf16(x-hi) at data + plane_stride elements; x ~ hi+lo, 16 mantissa bits).
- * cstride = elements between consecutive pixels, coffset = first channel used. */
+ * cstride = elements between consecutive pixels, coffset = first channel used.
+ * Split holds finite values only: +-inf stored as split loads back as NaN (hi = inf, lo = bf16(inf - inf) = NaN). */
 #define HEAL_FMT_F32 0
 #define HEAL_FMT_BF16 1
 #define HEAL_FMT_SPLIT 2
@@ -115,7 +116,10 @@ int heal_sparse_stem_tc(const float* pillar_features, const int* idmap, int batc
  *   weight: groups==1 : fp32 [kh][kw][Cin][w_cstride] (w_cstride >= Cout, multiple of 4), BN scale folded
  *           groups>1  : fp32 [kh*kw][Cin/groups][Cout/groups][groups] (3x3 only, Cin==Cout)
  *   output pixel (oh,ow) of the (Ho,Wo) conv grid is stored at (oh*upsample+up_i, ow*upsample+up_j)
- *   of an (Ho*upsample, Wo*upsample) map: a k==stride transposed conv is upsample^2 1x1 launches. */
+ *   of an (Ho*upsample, Wo*upsample) map: a k==stride transposed conv is upsample^2 1x1 launches.
+ *   in is read 4 channels at a time: Cin, in->cstride, in->coffset (and the split plane stride) multiples of 4 and in->data
+ *   16-byte aligned (fp32) or 8-byte aligned (bf16 / split), else HEAL_ERR_UNSUPPORTED.  The grouped conv writes 4 channels
+ *   at a time and refuses an out view that fails the same rule; the dense conv writes such a view one channel at a time. */
 int heal_conv2d_simt(const heal_act_t* in, int N, int H, int W, int Cin,
                      const float* weight, int w_cstride, const float* bias,
                      int kh, int kw, int stride, int pad, int groups,
@@ -269,7 +273,7 @@ int heal_swap_attention(const heal_act_t* qkv, const int* n_agents_host, int B, 
 
 /* Mean over n_avg consecutive images, then LayerNorm over the channels (biased variance, eps):
  * out image o = LayerNorm(mean_{k < n_avg} in image o*n_avg + k) for o < n_out.  n_avg = 1 is a plain LayerNorm.
- * ln_weight, ln_bias: (C) fp32 device.  C in {64, 128, 192, 256}. */
+ * ln_weight, ln_bias: (C) fp32 device.  C in {64, 128, 192, 256}.  n_out = 0 launches nothing (in / out data may be NULL). */
 int heal_mean_layernorm(const heal_act_t* in, int n_out, int n_avg, int H, int W, int C, const float* ln_weight,
                         const float* ln_bias, float eps, const heal_act_t* out, void* stream);
 
@@ -475,13 +479,18 @@ int heal_eval_tp_fp(const float* det_corners, const float* det_scores, int K, co
                     const float* thresholds_host, int n_thr, float* sorted_scores_out, unsigned char* tp_out, int* status_out,
                     void* ws, size_t ws_bytes, void* stream);
 
-/* ---- format conversion between fp32 and (split-)bf16 channels-last buffers ------------------- */
+/* ---- format conversion between fp32 and (split-)bf16 channels-last buffers -------------------
+ * Any views: 4 channels at a time when channels, both channel strides and offsets (and split plane strides) are multiples of 4
+ * and both data pointers are 16-byte aligned (fp32) or 8-byte aligned (bf16 / split), one channel at a time otherwise (same
+ * results).  fp32 -> bf16 rounds to nearest even; fp32 -> split is hi = bf16(x), lo = bf16(x - hi); split -> fp32 is hi + lo.
+ * num_pixels = 0 launches nothing (the data pointers may be NULL). */
 int heal_act_convert(const heal_act_t* src, const heal_act_t* dst, size_t num_pixels, int channels, void* stream);
 
 /* ---- ConvNeXt aligner (SURVEY.md 8f-3) -------------------------------------------------------------
  * depthwise k x k conv (+bias) + LayerNorm over channels, one kernel: the front half of ConvNeXtBlock.forward
  * (opencood/models/sub_modules/feature_alignnet_modules.py:331-336, LayerNorm :12-25 channels_last, biased variance).
- *   dw_weight [k*k][C] fp32 (tap-major), dw_bias [C] or NULL, ln_weight / ln_bias [C]; C in {64,128,192,256}
+ *   dw_weight [k*k][C] fp32 (tap-major, read as float2: 8-byte aligned, else HEAL_ERR_UNSUPPORTED), dw_bias [C] or NULL,
+ *   ln_weight / ln_bias [C]; C in {64,128,192,256}
  * The two Linear layers that follow are 1x1 convolutions on heal_conv2d_tc (`relu` = 2 selects the exact erf GELU in the
  * epilogue; layer scale `gamma` folded into the second one; the block's residual add is the conv's residual input). */
 int heal_dwconv_layernorm(const heal_act_t* in, int N, int H, int W, int C, const float* dw_weight, const float* dw_bias,
@@ -489,7 +498,9 @@ int heal_dwconv_layernorm(const heal_act_t* in, int N, int H, int W, int C, cons
 
 /* 3x3 / stride 2 / pad 1 max pooling, channels-last (torchvision ResNet stem of CamEncode_Resnet101,
  * opencood/models/sub_modules/lss_submodule.py:196-199).  depth_to_space_in != 0: the logical (N,H,W,C) input is stored as
- * (N,H/2,W/2,4C) with channel block (y&1)*2+(x&1) -- the phase-major output of the space-to-depth form of the 7x7/2 stem conv. */
+ * (N,H/2,W/2,4C) with channel block (y&1)*2+(x&1) -- the phase-major output of the space-to-depth form of the 7x7/2 stem conv.
+ * Reads and writes 4 channels at a time: C, channel strides, offsets (and split plane strides) multiples of 4 and in->data /
+ * out->data 16-byte aligned (fp32) or 8-byte aligned (bf16 / split), else HEAL_ERR_UNSUPPORTED. */
 int heal_maxpool3x3s2(const heal_act_t* in, int N, int H, int W, int C, int depth_to_space_in, const heal_act_t* out, void* stream);
 
 /* ---- EfficientNet-B0 camera trunk of Lift-Splat-Shoot (`camera_encoder: EfficientNet`, SURVEY.md 8c) ---------------------
