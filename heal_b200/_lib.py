@@ -18,6 +18,11 @@ class HealAct(ctypes.Structure):
 _ap = ctypes.POINTER(HealAct)
 
 
+class HealStackSource(ctypes.Structure):
+    """heal_stack_source_t of include/heal_b200.h"""
+    _fields_ = [("map", HealAct), ("images", _i), ("height", _i), ("width", _i), ("center_crop", _i)]
+
+
 class HealCavHeads(ctypes.Structure):
     """heal_cav_heads_t of include/heal_b200.h"""
     _fields_ = [("cls", _ap), ("reg", _ap), ("dir", _ap), ("iou", _ap), ("anchors", _vp), ("transform4x4_host", ctypes.POINTER(ctypes.c_float))]
@@ -60,6 +65,7 @@ SIGNATURES = {
     "heal_split_attn": (_i, [_ap, _ap, _i, _i, _i, _i, _vp, _vp, _vp, _c.c_float, _vp, _vp, _sz, _ap, _vp]),
     "heal_sttf_resample": (_i, [_ap, _vp, _i, _i, _i, _i, _ap, _vp]),
     "heal_act_convert": (_i, [_ap, _ap, _sz, _i, _vp]),
+    "heal_agent_stack": (_i, [ctypes.POINTER(HealStackSource), _i, _vp, _vp, _i, _i, _ap, _i, _i, _vp]),
     "heal_postprocess_workspace": (_sz, [_i, _i, _i, _i]),
     "heal_box_decode_nms": (_i, [_ap, _ap, _ap, _vp, _i, _i, _i, _c.c_float, _c.c_float, _i, _vp, _i, _c.c_float, _i,
                                  _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),

@@ -6,7 +6,6 @@ layer0 included, which the reference builds but never runs) and forward(data_dic
 import importlib
 from collections import OrderedDict, Counter
 
-import torch
 import torch.nn as nn
 
 from .. import ops
@@ -16,7 +15,7 @@ from .sub_modules.base_bev_backbone_resnet import ResNetBEVBackbone
 from .sub_modules.feature_alignnet import AlignNet
 from .sub_modules.downsample_conv import DownsampleConv
 from .fuse_modules.fusion_in_one import AttFusion, MaxFusion
-from .heter_pyramid_collab import FusedHeads, HeterPyramidCollab
+from .heter_pyramid_collab import FusedHeads
 
 
 class HeterModelBaselineMs(nn.Module):
@@ -97,7 +96,7 @@ class HeterModelBaselineMs(nn.Module):
         affine = normalize_pairwise_tfm(data_dict['pairwise_t_matrix'], self.H, self.W, self.fake_voxel_size)
         record_len = data_dict['record_len']
         count = Counter(aml)
-        feats = {}
+        feats, crops = {}, {}
         for m in self.modality_name_list:
             if m not in count:
                 continue
@@ -107,20 +106,14 @@ class HeterModelBaselineMs(nn.Module):
             f = bb.decode_nhwc(bb.multiscale_nhwc(f))
             f = getattr(self, f"aligner_{m}").forward_nhwc(f)
             if self.sensor_type_dict[m] == "camera":
-                f = HeterPyramidCollab._center_crop_nhwc(f, int(f.H * getattr(self, f"crop_ratio_H_{m}")),
-                                                         int(f.W * getattr(self, f"crop_ratio_W_{m}")))
+                crops[m] = (int(f.H * getattr(self, f"crop_ratio_H_{m}")), int(f.W * getattr(self, f"crop_ratio_W_{m}")))
                 if getattr(self, f"depth_supervision_{m}"):
                     output_dict[f"depth_items_{m}"] = enc.depth_items
             feats[m] = f
-        if len(feats) == 1 and all(a == aml[0] for a in aml):
+        if len(feats) == 1 and all(a == aml[0] for a in aml) and not crops:
             x = feats[aml[0]]
-        else:
-            cnt = {m: 0 for m in self.modality_name_list}
-            rows = []
-            for m in aml:
-                rows.append(ops.convert(feats[m].image(cnt[m]), "f32").t)
-                cnt[m] += 1
-            x = ops.Act(torch.cat(rows, 0), "f32")
+        else:                                   # fp32 (n_agents, H, W, C) in scene order, camera maps cropped / padded
+            x = ops.agent_stack(feats, aml, crops)
         if x.C != self.level_channels[0]:
             raise ValueError(f"the per-agent maps have {x.C} channels, the first fusion level {self.level_channels[0]}")
         if self.supervise_single:

@@ -135,7 +135,7 @@ class HeterPyramidCollab(nn.Module):
         affine = normalize_pairwise_tfm(data_dict['pairwise_t_matrix'], self.H, self.W, self.fake_voxel_size)
         record_len = data_dict['record_len']
         count = Counter(aml)
-        feats = {}
+        feats, crops = {}, {}
         for m in self.modality_name_list:
             if m not in count:
                 continue
@@ -145,20 +145,14 @@ class HeterPyramidCollab(nn.Module):
             f = bb.decode_nhwc(bb.multiscale_nhwc(f))                             # Act
             f = getattr(self, f"aligner_{m}").forward_nhwc(f)                     # identity, or the ConvNeXt aligner (HEAL stage 2)
             if self.sensor_type_dict[m] == "camera":
-                f = self._center_crop_nhwc(f, int(f.H * getattr(self, f"crop_ratio_H_{m}")),
-                                           int(f.W * getattr(self, f"crop_ratio_W_{m}")))
+                crops[m] = (int(f.H * getattr(self, f"crop_ratio_H_{m}")), int(f.W * getattr(self, f"crop_ratio_W_{m}")))
                 if getattr(self, f"depth_supervision_{m}"):
                     output_dict[f"depth_items_{m}"] = getattr(self, f"encoder_{m}").depth_items
             feats[m] = f
-        if len(feats) == 1 and all(a == aml[0] for a in aml):
+        if len(feats) == 1 and all(a == aml[0] for a in aml) and not crops:
             x = feats[aml[0]]
-        else:
-            cnt = {m: 0 for m in self.modality_name_list}
-            rows = []
-            for m in aml:
-                rows.append(ops.convert(feats[m].image(cnt[m]), "f32").t)
-                cnt[m] += 1
-            x = ops.Act(torch.cat(rows, 0), "f32")
+        else:                                   # fp32 (n_agents, H, W, C) in scene order, camera maps cropped / padded
+            x = ops.agent_stack(feats, aml, crops)
         if self.compress:
             x = self.compressor.forward_nhwc(x)
         fused, occs = self.pyramid_backbone.forward_collab_nhwc(x, record_len, affine, aml, self.cam_crop_info)

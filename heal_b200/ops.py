@@ -248,6 +248,47 @@ def convert(a: Act, fmt: str, out: Optional[Act] = None) -> Act:
     return out
 
 
+def _first_map(feats, *args, **kwargs):
+    return next(iter(feats.values()), None)
+
+
+@_guard(device_arg=_first_map)
+def agent_stack(feats: dict, agent_modality_list: Sequence[str], crops: Optional[dict] = None, fmt: str = "f32",
+                out: Optional[Act] = None) -> Act:
+    """The (n_agents, H, W, C) map of a heterogeneous scene in scene order, one heal_agent_stack launch: agent i is the next
+    image of `feats[agent_modality_list[i]]` (an Act per modality, any format).  `crops[m] = (th, tw)` center-crops or zero-pads
+    modality m's maps as torchvision CenterCrop does (the camera modalities); every other modality's maps must already have
+    the scene's size.  The result is in `fmt`: 'f32' is the hand-off the heterogeneous models' forwards use."""
+    crops = crops or {}
+    mods = list(dict.fromkeys(agent_modality_list))
+    sizes = {m: tuple(crops[m]) if m in crops else (feats[m].H, feats[m].W) for m in mods}
+    H, W = next((sizes[m] for m in mods if m not in crops), sizes[mods[0]])
+    C = feats[mods[0]].C
+    for m in mods:
+        f = feats[m]
+        if sizes[m] != (H, W) or f.C != C:
+            raise ValueError(f"agent_stack: {m} gives {f.C}-channel {sizes[m][0]}x{sizes[m][1]} maps, the scene is "
+                             f"{C}-channel {H}x{W}")
+        if agent_modality_list.count(m) > f.N:
+            raise ValueError(f"agent_stack: {agent_modality_list.count(m)} {m} agents, {f.N} {m} maps")
+    from ._lib import HealStackSource
+    srcs = (HealStackSource * len(mods))(*[HealStackSource(feats[m].view(), feats[m].N, feats[m].H, feats[m].W, int(m in crops))
+                                           for m in mods])
+    seen = {m: 0 for m in mods}
+    src_of, img_of = [], []
+    for m in agent_modality_list:
+        src_of.append(mods.index(m))
+        img_of.append(seen[m])
+        seen[m] += 1
+    n = len(agent_modality_list)
+    out = _out_act(out, n, H, W, C, fmt, feats[mods[0]].device)
+    assert out.fmt == fmt
+    nbytes = sum(H * W * float(C) * (BPE[feats[m].fmt] + BPE[fmt]) for m in agent_modality_list)
+    with _Prof("agent_stack", 0, nbytes):
+        _call("heal_agent_stack", srcs, len(mods), _host_i32(src_of), _host_i32(img_of), n, C, out.view(), H, W)
+    return out
+
+
 def to_nhwc(x: torch.Tensor) -> torch.Tensor:
     """(N,C,H,W) logical tensor -> contiguous (N,H,W,C) buffer (view if already channels-last)."""
     assert x.dim() == 4

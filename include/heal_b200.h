@@ -486,6 +486,30 @@ int heal_eval_tp_fp(const float* det_corners, const float* det_scores, int K, co
  * num_pixels = 0 launches nothing (the data pointers may be NULL). */
 int heal_act_convert(const heal_act_t* src, const heal_act_t* dst, size_t num_pixels, int channels, void* stream);
 
+/* ---- agent assembly of a heterogeneous scene ------------------------------------------------------
+ * replaces the per-agent convert + camera CenterCrop + torch.cat of HeterPyramidCollab / HeterModelBaseline /
+ * HeterModelBaselineMs.forward (heter_pyramid_collab.py:147-161, heter_model_baseline.py:117-130,
+ * heter_model_baseline_ms.py:110-123): agent a of the (num_agents, H, W, channels) `dst` is image agent_image_host[a] of source
+ * agent_source_host[a].  One source per modality: its (images, height, width, channels) map in any format.  A source with
+ * center_crop = 0 must be H x W and is copied; with center_crop = 1 it is cut to H x W as torchvision CenterCrop does: per axis
+ * of source size s and target t, zero padding of (t - s) // 2 before and (t - s + 1) // 2 after when t > s, else a window at
+ * int(round((s - t) / 2.0)) (Python rounding, halves to even).  Values are converted exactly as heal_act_convert converts
+ * them (dst in any format; padding is +0).  Sources, positions and sizes are host metadata copied into the launch, so the call
+ * can be captured.  4 channels at a time when channels and every view meet heal_act_convert's vector rule, one channel at a
+ * time otherwise (same results).  1 <= num_sources <= 8 and 1 <= num_agents <= 64 (HEAL_ERR_UNSUPPORTED above); a NULL data
+ * pointer, a format outside 0..2, cstride < coffset + channels, an agent index out of range or a center_crop = 0 source of
+ * another size is HEAL_ERR_ARG. */
+#define HEAL_AGENT_STACK_MAX_SOURCES 8
+#define HEAL_AGENT_STACK_MAX_AGENTS 64
+typedef struct {
+    heal_act_t map;
+    int images, height, width;
+    int center_crop;
+} heal_stack_source_t;
+int heal_agent_stack(const heal_stack_source_t* sources_host, int num_sources, const int* agent_source_host,
+                     const int* agent_image_host, int num_agents, int channels, const heal_act_t* dst, int H, int W,
+                     void* stream);
+
 /* ---- ConvNeXt aligner (SURVEY.md 8f-3) -------------------------------------------------------------
  * depthwise k x k conv (+bias) + LayerNorm over channels, one kernel: the front half of ConvNeXtBlock.forward
  * (opencood/models/sub_modules/feature_alignnet_modules.py:331-336, LayerNorm :12-25 channels_last, biased variance).
