@@ -48,6 +48,8 @@ SIGNATURES = {
                             _vp, _sz, _vp, _i, _i, _vp, _sz, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "heal_conv3x3_narrow_tc": (_i, [_ap, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _ap, _vp]),
     "heal_bottleneck_tc": (_i, [_vp, _sz, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _sz, _i, _i, _vp]),
+    "heal_gconv_reduce_tc": (_i, [_vp, _sz, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _sz, _i, _i, _i, _vp, _sz, _i, _i,
+                                  _vp]),
     "heal_dwconv_layernorm": (_i, [_ap, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _c.c_float, _ap, _vp]),
     "heal_maxpool3x3s2": (_i, [_ap, _i, _i, _i, _i, _i, _ap, _vp]),
     "heal_pyramid_fuse_level": (_i, [_ap, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _ap, _vp]),

@@ -85,11 +85,26 @@ class Bottleneck(nn.Module):
                 and c1.in_channels == x.C == c3.out_channels == 64 and c1.out_channels == c2.out_channels == c3.in_channels == 128
                 and c2.in_channels == 128)
 
+    def _gconv_reduce_eligible(self, x) -> bool:
+        """The shapes ops.gconv_reduce_tc runs after the expand: PyramidFusion's stride-1 level-1 and level-2 blocks
+        (C -> 2 C -> C with C = 128 or 256, 32 groups, no downsample)."""
+        from ... import engine
+        c1, c2, c3 = self.conv1, self.conv2, self.conv3
+        return (isinstance(x, ops.Act) and x.fmt == engine.act_fmt() and engine.PRECISION in ("tc32", "bf16")
+                and not engine.BF16_WEIGHTS and self.downsample is None and c2.stride == (1, 1) and c2.groups == 32
+                and x.C == c1.in_channels == c3.out_channels and x.C in (128, 256)
+                and c1.out_channels == c2.in_channels == c2.out_channels == c3.in_channels == 2 * x.C)
+
     def forward_nhwc(self, x, out=None):
         if self._fused_eligible(x) and (out is None or out.fmt == x.fmt):
             from ... import engine
             pcs = [engine.packed(c, b, True, kind="tc2") for c, b in ((self.conv1, self.bn1), (self.conv2, self.bn2), (self.conv3, self.bn3))]
             return ops.bottleneck_tc(x, *pcs, out=out)
+        if self._gconv_reduce_eligible(x) and (out is None or out.fmt == x.fmt):
+            from ... import engine
+            y = conv_bn_act(x, self.conv1, self.bn1, relu=True)
+            pc2, pc3 = (engine.packed(c, b, True, kind="tc2") for c, b in ((self.conv2, self.bn2), (self.conv3, self.bn3)))
+            return ops.gconv_reduce_tc(y, pc2, pc3, x, out=out)
         idt = x
         if self.downsample is not None:
             idt = conv_bn_act(x, self.downsample[0], self.downsample[1], relu=False)

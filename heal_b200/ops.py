@@ -790,6 +790,33 @@ def bottleneck_tc(x: Act, pc1: PackedConvTC, pc2: PackedConvTC, pc3: PackedConvT
     return out
 
 
+@_guard
+def gconv_reduce_tc(mid: Act, pc2: PackedConvTC, pc3: PackedConvTC, residual: Act, out: Optional[Act] = None,
+                    out_coffset: int = 0) -> Act:
+    """ReLU(conv3(conv2(mid)) + residual) of a stride-1 ResNeXt bottleneck (grouped 3x3 width -> width, 1x1 width -> C) in one
+    kernel: bit-identical to conv2d_tc(pc2) -> conv2d_tc(pc3, residual=residual).  mid, residual: Acts 'split' or 'bf16' of the
+    same format; the packed weights carry both planes.  `out` (optional, that format): written at channels
+    [out_coffset, out_coffset + C)."""
+    _need_cuda(pc2.w_diag, pc3.w)
+    assert mid.planes in (1, 2) and residual.fmt == mid.fmt and pc2.planes == pc3.planes == 2
+    assert pc2.blockdiag and pc2.kh == 3 and pc2.stride == 1 and pc2.cin == pc2.cout == mid.C
+    assert (pc3.kh, pc3.cin, pc3.cout, pc3.coutp) == (1, mid.C, residual.C, residual.C)
+    N, H, W, C, width = mid.N, mid.H, mid.W, residual.C, mid.C
+    assert (residual.N, residual.H, residual.W) == (N, H, W)
+    if out is None:
+        out = act_empty(N, H, W, C, mid.fmt, mid.device)
+    assert out.fmt == mid.fmt and (out.N, out.H, out.W) == (N, H, W) and out_coffset + C <= out.C
+    flops = 2.0 * N * H * W * (width * (width // pc2.groups) * 9 + width * C)
+    epb = 2.0 * mid.planes
+    nbytes = N * H * W * (width + 2.0 * C) * epb + 2.0 * (pc2.w_diag.numel() + pc3.w.numel())
+    with _Prof("conv_tc_gconv_reduce", flops, nbytes):
+        _call("heal_gconv_reduce_tc", _p(mid.t), mid.plane_stride, N, H, W, width, mid.cstride,
+              _p(pc2.w_diag), _p(pc2.bias), _p(pc3.w), _p(pc3.bias), C,
+              _p(residual.t), residual.plane_stride, residual.cstride, mid.planes, pc3.planes,
+              _p(out.t), out.plane_stride, out.cstride, out_coffset)
+    return out
+
+
 # ------------------------------------------------------------------------------------------------
 # ConvNeXt aligner front half, ResNet-stem max pooling
 # ------------------------------------------------------------------------------------------------

@@ -182,6 +182,18 @@ int heal_bottleneck_tc(const void* x, size_t x_plane_stride, int N, int H, int W
                        const void* w1, const float* b1, const void* w2_diag, const float* b2, const void* w3, const float* b3,
                        int planes, int w_planes, void* out, size_t out_plane_stride, int out_cstride, int out_coffset, void* stream);
 
+/* ---- ResNeXt bottleneck, grouped 3x3 + 1x1 reduce fused (PyramidFusion levels 1 and 2) -------------
+ * y = ReLU(conv3(ReLU(conv2(mid))) + res) for the stride-1 Bottleneck's grouped 3x3 (32 groups, width channels) and 1x1 reduce
+ * (width -> Cout) with the identity residual, as one kernel: the grouped conv's output stays on chip.  mid is the expand's
+ * output (N,H,W,width), res the block input (N,H,W,Cout).  The weights are the packings heal_conv2d_tc takes for those convs
+ * (w_planes = 2): w2_diag [2][9*width][16] (the diagonal sub-blocks of the grouped conv), w3 [2][Cout][width]; biases fp32.
+ * width a multiple of 64, Cout a multiple of 128; planes 2 (split-bf16) or 1 (bf16).  The output is bit-identical to the two
+ * heal_conv2d_tc launches and may be a channel slice [out_coffset, out_coffset + Cout) of a wider map. */
+int heal_gconv_reduce_tc(const void* mid, size_t mid_plane_stride, int N, int H, int W, int width, int mid_cstride,
+                         const void* w2_diag, const float* b2, const void* w3, const float* b3, int Cout,
+                         const void* res, size_t res_plane_stride, int res_cstride, int planes, int w_planes,
+                         void* out, size_t out_plane_stride, int out_cstride, int out_coffset, void* stream);
+
 /* ---- PyramidFusion weighted fuse of one level -------------------------------------------------
  * replaces weighted_fuse (opencood/models/fuse_modules/pyramid_fuse.py:17-63) incl. both
  * warp_affine_simple calls (torch_transformation_utils.py:323-332), score = sigmoid(occ)+1e-4
