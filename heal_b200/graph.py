@@ -7,6 +7,7 @@ travels in `agent_offsets[-1]` on the device, so clouds of different sizes reuse
 """
 from __future__ import annotations
 
+import collections
 import numbers
 
 import torch
@@ -190,22 +191,41 @@ class FramePipeline:
         return pipe
 
     def _start(self, graphs, results, dev, compute_streams):
-        """`results[k]`: the device tensors slot k copies back to the host after each replay, by name."""
+        """`results[k]`: the device tensors slot k copies back to the host after each replay, by name (None: bound later by
+        `_bind`, when the slot's first graph exists)."""
         self.dev, self.depth = dev, len(graphs)
-        self.graphs, self.dev_out = graphs, results
+        self.graphs = graphs
         self.s_in, self.s_out = (torch.cuda.Stream(device=dev) for _ in range(2))
         comp = [torch.cuda.Stream(device=dev) for _ in range(2 if compute_streams >= 2 else 1)]
         self.s_comp = comp                                     # consecutive frames alternate between the compute streams
         self.ev_in = [torch.cuda.Event() for _ in range(self.depth)]
         self.ev_comp = [torch.cuda.Event() for _ in range(self.depth)]
         self.ev_out = [torch.cuda.Event() for _ in range(self.depth)]
-        self.host_out = [{k: torch.empty(t.shape, dtype=t.dtype).pin_memory() for k, t in r.items()} for r in results]
+        self.dev_out, self.host_out = [None] * self.depth, [None] * self.depth
         self.count = 0
         self.h2d_bytes = 0
-        self.d2h_bytes = sum(t.numel() * t.element_size() for t in self.host_out[0].values())
+        self.d2h_bytes = 0
+        for k, r in enumerate(results):
+            if r is not None:
+                self._bind(k, r)
         cur = torch.cuda.current_stream(dev)
         for s in (self.s_in, *set(self.s_comp), self.s_out):
             s.wait_stream(cur)
+
+    def _bind(self, k, results):
+        """Slot k copies `results` (device tensors by name) into its pinned host tensors after each replay."""
+        self.dev_out[k] = results
+        if self.host_out[k] is None:
+            self.host_out[k] = {n: torch.empty(t.shape, dtype=t.dtype).pin_memory() for n, t in results.items()}
+            self.d2h_bytes = sum(t.numel() * t.element_size() for t in self.host_out[k].values())
+
+    def _slot(self, k, *inputs):
+        """The graph slot k replays for this frame."""
+        return self.graphs[k]
+
+    def _result(self, k):
+        """What `submit` / `drain` hand back for the frame that last used slot k."""
+        return self.host_out[k]
 
     def submit(self, points: torch.Tensor, offsets: torch.Tensor, pairwise: torch.Tensor):
         return self._submit(points, offsets, pairwise)
@@ -213,7 +233,7 @@ class FramePipeline:
     def _submit(self, *inputs):
         d = self.depth
         k = self.count % d
-        g = self.graphs[k]
+        g = self._slot(k, *inputs)
         prev = None
         with torch.cuda.stream(self.s_in):
             if self.count >= d:
@@ -235,7 +255,7 @@ class FramePipeline:
         if self.count >= d - 1:
             j = (self.count - (d - 1)) % d
             self.ev_out[j].synchronize()                       # frame count-(depth-1) is complete on the host
-            prev = self.host_out[j]
+            prev = self._result(j)
         self.h2d_bytes = h2d
         self.count += 1
         return prev
@@ -245,7 +265,7 @@ class FramePipeline:
         out = []
         for c in range(max(self.count - (self.depth - 1), 0), self.count):
             self.ev_out[c % self.depth].synchronize()
-            out.append(self.host_out[c % self.depth])
+            out.append(self._result(c % self.depth))
         return out
 
     def flush(self):
@@ -315,6 +335,40 @@ def _input_buffers(spec, dev):
             inputs[m] = {"points": torch.zeros((sp["lidar"], 4), dtype=torch.float32, device=dev),
                          "agent_offsets": torch.zeros((k + 1,), dtype=torch.int32, device=dev)}
     return inputs
+
+
+def _input_views(spec, inputs):
+    """The input buffers of `spec` as leading slices of caller-owned ones (`_input_buffers` of the same capacities for as many or
+    more agents), so that the graphs of several agent lists can read one set.  Raises ValueError for a buffer that cannot hold
+    the spec's."""
+    views = {}
+    for m, want in _input_buffers(spec, "meta").items():
+        views[m] = {}
+        for key, w in want.items():
+            b = inputs.get(m, {}).get(key)
+            if b is None or b.dtype != w.dtype or b.shape[1:] != w.shape[1:] or b.shape[0] < w.shape[0]:
+                got = "missing" if b is None else f"{tuple(b.shape)} {b.dtype}"
+                raise ValueError(f"inputs[{m!r}][{key!r}]: {got}, the scene needs {tuple(w.shape)} {w.dtype}")
+            views[m][key] = b[:w.shape[0]]
+    return views
+
+
+def _voxel_limits(model, spec, voxel_limits):
+    """{m: {max_points_per_voxel, max_voxels}} of every lidar modality of `spec`: the encoder's defaults unless `voxel_limits[m]`
+    gives them."""
+    out = {}
+    for m, sp in spec.items():
+        if "lidar" in sp:
+            lim = dict(getattr(model, f"encoder_{m}").voxelize_args)
+            lim.update((voxel_limits or {}).get(m, {}))
+            out[m] = {k: int(lim[k]) for k in ("max_points_per_voxel", "max_voxels")}
+    return out
+
+
+def _anchor_box(postprocess_params):
+    """The anchors (H, W, A, 7) of VoxelPostprocessor for `postprocess_params`, on the host."""
+    from .data_utils.post_processor.voxel_postprocessor import VoxelPostprocessor
+    return VoxelPostprocessor(postprocess_params, False).generate_anchor_box()
 
 
 class LateFusionGraph:
@@ -465,33 +519,33 @@ class SceneGraph:
     (cameras, frame height, frame width, torch.uint8) for raw frames, which the encoder resizes, crops and normalises on the
     GPU.  The voxelisation limits of a lidar modality are the encoder's defaults unless `voxel_limits[m]` gives
     {max_points_per_voxel, max_voxels}; a batch that carries other values is refused.  The ego's boxes are decoded in the ego
-    frame (intermediate fusion: the identity transform)."""
+    frame (intermediate fusion: the identity transform).
+
+    Several graphs can share memory (SceneStream does so per pipeline slot): `inputs` are caller-owned input buffers, as
+    `_input_buffers` makes them for these capacities and as many or more agents (the graph reads leading slices);
+    `postprocess_buffers` are caller-owned ops.PostprocessBuffers for the box decode; `pool` is the private memory pool the frame
+    is captured into (torch.cuda.graph_pool_handle()).  The warm-up frames run outside the pool, so weight caches built lazily
+    land in the ordinary allocator."""
 
     def __init__(self, model, agent_modality_list, capacities, pairwise_shape, postprocess_params=None, device=None,
-                 voxel_limits=None, warmup: int = 2, top: int = 1000):
+                 voxel_limits=None, warmup: int = 2, top: int = 1000, inputs=None, pool=None, postprocess_buffers=None):
         from . import ops
         dev = device or next(model.parameters()).device
         self.modalities = list(agent_modality_list)
         n = len(self.modalities)
         self.spec = scene_spec(model.sensor_type_dict, self.modalities, capacities)
-        self.inputs = _input_buffers(self.spec, dev)
-        self.voxel_limits = {}
-        for m, sp in self.spec.items():
-            if "lidar" in sp:
-                lim = dict(getattr(model, f"encoder_{m}").voxelize_args)
-                lim.update((voxel_limits or {}).get(m, {}))
-                self.voxel_limits[m] = {k: int(lim[k]) for k in ("max_points_per_voxel", "max_voxels")}
-                self.inputs[m].update(self.voxel_limits[m])
+        self.inputs = _input_buffers(self.spec, dev) if inputs is None else _input_views(self.spec, inputs)
+        self.voxel_limits = _voxel_limits(model, self.spec, voxel_limits)
+        for m, lim in self.voxel_limits.items():
+            self.inputs[m].update(lim)
         self.pairwise = torch.eye(4, dtype=torch.float64, device=dev).expand(tuple(pairwise_shape)).contiguous()
         self.data = {**{f"inputs_{m}": buf for m, buf in self.inputs.items()}, "agent_modality_list": list(self.modalities),
                      "record_len": [n], "pairwise_t_matrix": self.pairwise}
         self.postprocess = None
         if postprocess_params is not None:
-            from .data_utils.post_processor.voxel_postprocessor import VoxelPostprocessor
-            pp = VoxelPostprocessor(postprocess_params, False)
-            self.anchors = torch.from_numpy(pp.generate_anchor_box()).to(device=dev, dtype=torch.float32).contiguous()
+            self.anchors = torch.from_numpy(_anchor_box(postprocess_params)).to(device=dev, dtype=torch.float32).contiguous()
             H, W, A = self.anchors.shape[:3]
-            self.postprocess = ops.PostprocessBuffers(H, W, A, top, dev)
+            self.postprocess = ops.PostprocessBuffers(H, W, A, top, dev) if postprocess_buffers is None else postprocess_buffers
         pparams, eye = postprocess_params, torch.eye(4, dtype=torch.float64)
 
         def run():
@@ -514,7 +568,7 @@ class SceneGraph:
         torch.cuda.synchronize(dev)
         self.graph = torch.cuda.CUDAGraph()
         l0 = lib.heal_launch_count()
-        with torch.no_grad(), torch.cuda.graph(self.graph, capture_error_mode="thread_local"):
+        with torch.no_grad(), torch.cuda.graph(self.graph, pool=pool, capture_error_mode="thread_local"):
             self.out = run()
         self.kernels_per_replay = int(lib.heal_launch_count() - l0)
 
@@ -560,3 +614,138 @@ class ScenePipeline(FramePipeline):
 
     def submit(self, ego_batch):
         return self._submit(ego_batch)
+
+
+class SceneGraphCache:
+    """The host side of SceneStream: a frame's key and its refusals, and per pipeline slot the captured graphs by key, least
+    recently used first.  The key is the ordered `agent_modality_list` as a tuple (the ego first; the order is the fusion
+    order).  `capture(slot, key)` makes slot `slot`'s graph for `key`."""
+
+    def __init__(self, sensor_type_dict, capacities, max_cav: int, voxel_limits, slots: int, max_graphs: int, capture):
+        if int(max_graphs) < 1:
+            raise ValueError(f"max_graphs {max_graphs}: a slot keeps at least one graph")
+        self.sensors, self.capacities = dict(sensor_type_dict), dict(capacities)
+        self.max_cav, self.voxel_limits, self.max_graphs = int(max_cav), voxel_limits, int(max_graphs)
+        self.slots = [collections.OrderedDict() for _ in range(slots)]
+        self.capture = capture
+        self.captures = 0
+
+    def _spec(self, key):
+        if not 0 < len(key) <= self.max_cav:
+            raise ValueError(f"{len(key)} agents {list(key)}: the stream serves 1 to max_cav = {self.max_cav}")
+        return scene_spec(self.sensors, key, self.capacities)
+
+    def key(self, agent_modality_list):
+        """The key of an agent list.  Raises ValueError for an empty list, more agents than `max_cav`, a modality the model
+        does not have or one without a capacity."""
+        key = tuple(agent_modality_list)
+        self._spec(key)
+        return key
+
+    def check(self, ego_batch):
+        """The key of a collated `batch_data['ego']`, after the checks of `key` and of `check_scene` for the frame's own list
+        (host only, nothing is copied)."""
+        key = tuple(ego_batch["agent_modality_list"])
+        check_scene(self._spec(key), key, self.voxel_limits, ego_batch)
+        return key
+
+    def graph(self, slot: int, key):
+        """Slot `slot`'s graph for `key`, captured on a miss.  Above `max_graphs` the least recently used graph of the slot is
+        dropped, after the new one is captured, so the slot's memory pool always has a graph that holds it."""
+        graphs = self.slots[slot]
+        if key in graphs:
+            graphs.move_to_end(key)
+            return graphs[key]
+        g = graphs[key] = self.capture(slot, key)
+        self.captures += 1
+        while len(graphs) > self.max_graphs:
+            graphs.popitem(last=False)
+        return g
+
+    @property
+    def graphs_captured(self):
+        """Graphs held over all slots."""
+        return sum(len(s) for s in self.slots)
+
+
+class SceneStream(FramePipeline):
+    """A stream of mixed-modality scenes whose agent list changes from frame to frame (the CAVs in range and their modalities,
+    as in a dataset's test split), served through FramePipeline's slots: copy-in stream, compute stream, copy-out stream, events
+    and no host sync.  `submit(ego_batch)` returns, pinned on the host, frame i - (depth - 1): the ego's boxes, scores and box
+    count with `postprocess_params` (`boxes[:count[0]]`), else its heads, and the frame's `agent_modality_list`.
+
+        stream = SceneStream(model, {"m1": 240_000, "m2": (4, 600, 800, torch.uint8), "m3": 120_000, "m4": (4, 600, 800,
+                             torch.uint8)}, pairwise_shape=(1, 5, 5, 4, 4), postprocess_params=hypes["postprocess"])
+        for batch_data in data_loader:
+            res = stream.submit(batch_data["ego"])      # None while the pipeline fills
+        rest = stream.drain()
+
+    `capacities` follows SceneGraph for every modality the stream may see; `pairwise_shape[1]` is max_cav.  Each slot keeps one
+    captured SceneGraph per agent list, so a 2-agent frame runs a 2-agent graph and its result is bit for bit that of a
+    SceneGraph captured for its list alone.  A list new to a slot is captured inside `submit` (a device synchronise and two eager
+    warm-up frames); `capture(agent_modality_list)` does it ahead.  Above `max_graphs` graphs in a slot the least recently used
+    one is dropped (and recaptured if its list comes back).  A frame that cannot be served raises ValueError on the host before
+    anything is copied: a modality the model does not have or without a capacity, more agents than max_cav, or any refusal of
+    `check_scene` for its own list.
+
+    Memory: the graphs of slot k are captured into one private pool, read slot k's one set of input buffers (every modality at
+    its capacity, for max_cav agents) and write slot k's one set of post-processing buffers, which lie outside the pool.  Graphs
+    of one slot never run at once (slot k's next frame waits for its last one's replay and copy-out), so they share their
+    scratch.  A graph's static outputs may lie in another graph's scratch: a frame's device results are valid only until its
+    slot's next replay.  The copy-out to the host happens before that; the host results are valid until the slot's next
+    copy-out, `depth` submits later, as in FramePipeline."""
+
+    def __init__(self, model, capacities, pairwise_shape, postprocess_params=None, depth: int = 2, max_graphs: int = 16,
+                 voxel_limits=None, device=None):
+        from . import ops
+        dev = device or next(model.parameters()).device
+        depth = max(1, int(depth))
+        self.model, self.capacities, self.pairwise_shape = model, dict(capacities), tuple(pairwise_shape)
+        self.postprocess_params, self.voxel_limits = postprocess_params, voxel_limits
+        spec = scene_spec(model.sensor_type_dict, list(self.capacities), self.capacities)
+        max_cav = int(self.pairwise_shape[1])
+        self.cache = SceneGraphCache(model.sensor_type_dict, self.capacities, max_cav, _voxel_limits(model, spec, voxel_limits),
+                                     depth, max_graphs, self._capture)
+        self.inputs = [_input_buffers({m: dict(sp, agents=max_cav) for m, sp in spec.items()}, dev) for _ in range(depth)]
+        self.pools = [torch.cuda.graph_pool_handle() for _ in range(depth)]
+        self.postprocess = [None] * depth
+        if postprocess_params is not None:
+            H, W, A = _anchor_box(postprocess_params).shape[:3]
+            self.postprocess = [ops.PostprocessBuffers(H, W, A, 1000, dev) for _ in range(depth)]   # SceneGraph's `top`
+        self.lists = [None] * depth                             # the agent list of the frame that last used each slot
+        self._start(self.cache.slots, [None] * depth, dev, 2)
+
+    def _capture(self, k, key):
+        self.join(begin=False)          # the warm-up follows every frame in flight: slot k's last frame has left its buffers
+        return SceneGraph(self.model, list(key), self.capacities, self.pairwise_shape, self.postprocess_params, device=self.dev,
+                          voxel_limits=self.voxel_limits, inputs=self.inputs[k], pool=self.pools[k],
+                          postprocess_buffers=self.postprocess[k])
+
+    def _slot(self, k, ego_batch):
+        key = self.cache.check(ego_batch)
+        g = self.cache.graph(k, key)
+        self.lists[k] = key
+        self._bind(k, g.results())
+        return g
+
+    def _result(self, k):
+        return {**self.host_out[k], "agent_modality_list": list(self.lists[k])}
+
+    def submit(self, ego_batch):
+        return self._submit(ego_batch)
+
+    def capture(self, agent_modality_list):
+        """Capture the graphs of an agent list in every slot ahead of the stream (a list a slot already holds is kept)."""
+        key = self.cache.key(agent_modality_list)
+        for k in range(self.depth):
+            self.cache.graph(k, key)
+
+    @property
+    def captures(self):
+        """Graph captures so far, recaptures after eviction included."""
+        return self.cache.captures
+
+    @property
+    def graphs_captured(self):
+        """Graphs the stream holds over all slots."""
+        return self.cache.graphs_captured
