@@ -3,46 +3,35 @@
 every agent -> per-level fusion -> decode -> (shrink) -> heads.  Same ctor argument, state-dict keys (the fusion backbone's
 layer0 included, which the reference builds but never runs) and forward(data_dict) -> output_dict contract.
 `fusion_method`: att (AttFusion per level) and max (MaxFusion per level), the two the reference builds."""
-import importlib
-from collections import OrderedDict, Counter
+from collections import OrderedDict
 
 import torch.nn as nn
 
-from .. import ops
 from ..engine import require_eval
 from ..utils.transformation_utils import normalize_pairwise_tfm
 from .sub_modules.base_bev_backbone_resnet import ResNetBEVBackbone
 from .sub_modules.feature_alignnet import AlignNet
 from .sub_modules.downsample_conv import DownsampleConv
 from .fuse_modules.fusion_in_one import AttFusion, MaxFusion
-from .heter_pyramid_collab import FusedHeads
+from .heter_common import HeterFront, add_heads, modality_names
 
 
-class HeterModelBaselineMs(nn.Module):
+class HeterModelBaselineMs(HeterFront, nn.Module):
+    adapter_name = "aligner"
+
     def __init__(self, args):
         super().__init__()
         self.args = args
-        self.modality_name_list = [x for x in args.keys() if x.startswith("m") and x[1:].isdigit()]
+        self.modality_name_list = modality_names(args)
         self.ego_modality = args.get('ego_modality')
         self.stage2_added_modality = args.get('stage2_added_modality', None)
         self.cav_range = args['lidar_range']
         self.sensor_type_dict = OrderedDict()
-        encoder_lib = importlib.import_module("heal_b200.models.heter_encoders")
         for m in self.modality_name_list:
             setting = args[m]
-            self.sensor_type_dict[m] = setting['sensor_type']
-            target = setting['core_method'].replace('_', '').lower()
-            enc_cls = next((c for n, c in encoder_lib.__dict__.items() if n.lower() == target), None)
-            if enc_cls is None:
-                raise NotImplementedError(f"encoder '{setting['core_method']}' not available in heal_b200.models.heter_encoders")
-            setattr(self, f"encoder_{m}", enc_cls(setting['encoder_args']))
-            setattr(self, f"depth_supervision_{m}", bool(setting['encoder_args'].get("depth_supervision", False)))
-            setattr(self, f"backbone_{m}", ResNetBEVBackbone(setting['backbone_args']))
-            setattr(self, f"aligner_{m}", AlignNet(setting['aligner_args']))
+            self._add_modality(m, setting, ResNetBEVBackbone(setting['backbone_args']), AlignNet(setting['aligner_args']))
             if setting['sensor_type'] == "camera":
                 g = setting['camera_mask_args']['grid_conf']
-                setattr(self, f"crop_ratio_W_{m}", self.cav_range[3] / g['xbound'][1])
-                setattr(self, f"crop_ratio_H_{m}", self.cav_range[4] / g['ybound'][1])
                 setattr(self, f"xdist_{m}", g['xbound'][1] - g['xbound'][0])
                 setattr(self, f"ydist_{m}", g['ybound'][1] - g['ybound'][0])
         self.H = self.cav_range[4] - self.cav_range[1]
@@ -50,11 +39,7 @@ class HeterModelBaselineMs(nn.Module):
         self.fake_voxel_size = 1
         self.supervise_single = bool(args.get("supervise_single", False))
         if self.supervise_single:
-            c = args['in_head_single']
-            self.cls_head_single = nn.Conv2d(c, args['anchor_number'], kernel_size=1)
-            self.reg_head_single = nn.Conv2d(c, args['anchor_number'] * 7, kernel_size=1)
-            self.dir_head_single = nn.Conv2d(c, args['anchor_number'] * args['dir_args']['num_bins'], kernel_size=1)
-            self._heads_single = FusedHeads([self.cls_head_single, self.reg_head_single, self.dir_head_single])
+            self._heads_single = add_heads(self, args['in_head_single'], args, "_single")
 
         # fusion: one module per fusion-backbone level; level i has num_filters[i] channels
         self.backbone = ResNetBEVBackbone(args['fusion_backbone'])
@@ -81,39 +66,14 @@ class HeterModelBaselineMs(nn.Module):
         self.shrink_flag = 'shrink_header' in args
         if self.shrink_flag:
             self.shrink_conv = DownsampleConv(args['shrink_header'])
-        self.cls_head = nn.Conv2d(args['in_head'], args['anchor_number'], kernel_size=1)
-        self.reg_head = nn.Conv2d(args['in_head'], 7 * args['anchor_number'], kernel_size=1)
-        self.dir_head = nn.Conv2d(args['in_head'], args['dir_args']['num_bins'] * args['anchor_number'], kernel_size=1)
-        self._heads = FusedHeads([self.cls_head, self.reg_head, self.dir_head])
-
-    def model_train_init(self):
-        pass
+        self._heads = add_heads(self, args['in_head'], args)
 
     def forward(self, data_dict):
         require_eval(self)
         output_dict = {}
-        aml = data_dict['agent_modality_list']
         affine = normalize_pairwise_tfm(data_dict['pairwise_t_matrix'], self.H, self.W, self.fake_voxel_size)
         record_len = data_dict['record_len']
-        count = Counter(aml)
-        feats, crops = {}, {}
-        for m in self.modality_name_list:
-            if m not in count:
-                continue
-            enc = getattr(self, f"encoder_{m}")
-            f = enc.forward_act(data_dict, m) if hasattr(enc, "forward_act") else ops.to_act(enc(data_dict, m))
-            bb = getattr(self, f"backbone_{m}")
-            f = bb.decode_nhwc(bb.multiscale_nhwc(f))
-            f = getattr(self, f"aligner_{m}").forward_nhwc(f)
-            if self.sensor_type_dict[m] == "camera":
-                crops[m] = (int(f.H * getattr(self, f"crop_ratio_H_{m}")), int(f.W * getattr(self, f"crop_ratio_W_{m}")))
-                if getattr(self, f"depth_supervision_{m}"):
-                    output_dict[f"depth_items_{m}"] = enc.depth_items
-            feats[m] = f
-        if len(feats) == 1 and all(a == aml[0] for a in aml) and not crops:
-            x = feats[aml[0]]
-        else:                                   # fp32 (n_agents, H, W, C) in scene order, camera maps cropped / padded
-            x = ops.agent_stack(feats, aml, crops)
+        x = self._assemble(data_dict, output_dict)
         if x.C != self.level_channels[0]:
             raise ValueError(f"the per-agent maps have {x.C} channels, the first fusion level {self.level_channels[0]}")
         if self.supervise_single:

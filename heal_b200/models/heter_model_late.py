@@ -6,7 +6,6 @@ forward(data_dict) -> output_dict contract.
 `forward_late(batch_data)` runs a late-fusion batch (`{cav_id: cav_content}`, what the late datasets collate and
 `inference_late_fusion` loops over) as ONE batched forward per modality present; `LateForward` holds that part, which
 HeterPyramidSingle shares."""
-import importlib
 from collections import OrderedDict
 
 import torch
@@ -16,7 +15,7 @@ from .. import ops
 from ..engine import require_eval
 from .sub_modules.base_bev_backbone_resnet import ResNetBEVBackbone
 from .sub_modules.downsample_conv import DownsampleConv
-from .heter_pyramid_collab import FusedHeads, HeterPyramidCollab
+from .heter_common import HeterFront, add_heads, center_crop_nhwc, modality_names
 
 
 def modality_of(data_dict):
@@ -140,68 +139,28 @@ class LateForward:
         return out
 
 
-def build_encoder(setting):
-    encoder_lib = importlib.import_module("heal_b200.models.heter_encoders")
-    target = setting['core_method'].replace('_', '').lower()
-    enc_cls = next((c for n, c in encoder_lib.__dict__.items() if n.lower() == target), None)
-    if enc_cls is None:
-        raise NotImplementedError(f"encoder '{setting['core_method']}' not available in heal_b200.models.heter_encoders")
-    return enc_cls(setting['encoder_args'])
-
-
-def encode(model, data_dict, m):
-    """encoder -> backbone (resnet + deblocks) of modality m, as an Act (both single-agent models start so)."""
-    enc = getattr(model, f"encoder_{m}")
-    f = enc.forward_act(data_dict, m) if hasattr(enc, "forward_act") else ops.to_act(enc(data_dict, m))
-    bb = getattr(model, f"backbone_{m}")
-    return bb.decode_nhwc(bb.multiscale_nhwc(f))
-
-
-def crop_camera(model, f, m, extras):
-    """CenterCrop of a camera map to the lidar range (heter_model_late.py:79-89), and the depth items when supervised."""
-    if model.sensor_type_dict[m] != "camera":
-        return f
-    f = HeterPyramidCollab._center_crop_nhwc(f, int(f.H * getattr(model, f"crop_ratio_H_{m}")),
-                                             int(f.W * getattr(model, f"crop_ratio_W_{m}")))
-    if getattr(model, f"depth_supervision_{m}"):
-        extras[f"depth_items_{m}"] = getattr(model, f"encoder_{m}").depth_items
-    return f
-
-
-class HeterModelLate(LateForward, nn.Module):
+class HeterModelLate(LateForward, HeterFront, nn.Module):
     def __init__(self, args):
         super().__init__()
-        self.modality_name_list = [x for x in args.keys() if x.startswith("m") and x[1:].isdigit()]
+        self.modality_name_list = modality_names(args)
         self.cav_range = args['lidar_range']
         self.sensor_type_dict = OrderedDict()
         self._heads = {}
         for m in self.modality_name_list:
             setting = args[m]
-            self.sensor_type_dict[m] = setting['sensor_type']
-            setattr(self, f"encoder_{m}", build_encoder(setting))
-            setattr(self, f"depth_supervision_{m}", bool(setting['encoder_args'].get("depth_supervision", False)))
-            setattr(self, f"backbone_{m}", ResNetBEVBackbone(setting['backbone_args']))
-            if setting['sensor_type'] == "camera":
-                g = setting['camera_mask_args']['grid_conf']
-                setattr(self, f"crop_ratio_W_{m}", self.cav_range[3] / g['xbound'][1])
-                setattr(self, f"crop_ratio_H_{m}", self.cav_range[4] / g['ybound'][1])
+            self._add_modality(m, setting, ResNetBEVBackbone(setting['backbone_args']))
             setattr(self, f"layers_{m}", ResNetBEVBackbone(setting['layers_args']))
             setattr(self, f"layers_num_{m}", len(setting['layers_args']['num_upsample_filter']))
             setattr(self, f"shrink_conv_{m}", DownsampleConv(setting['shrink_header']))
-            in_head = setting['head_args']['in_head']
-            setattr(self, f"cls_head_{m}", nn.Conv2d(in_head, args['anchor_number'], kernel_size=1))
-            setattr(self, f"reg_head_{m}", nn.Conv2d(in_head, args['anchor_number'] * 7, kernel_size=1))
-            setattr(self, f"dir_head_{m}", nn.Conv2d(in_head, args['anchor_number'] * args['dir_args']['num_bins'], kernel_size=1))
-            self._heads[m] = FusedHeads([getattr(self, f"{h}_head_{m}") for h in ("cls", "reg", "dir")])
-
-    def model_train_init(self):
-        pass
+            self._heads[m] = add_heads(self, setting['head_args']['in_head'], args, f"_{m}")
 
     def _any_heads(self):
         return next(iter(self._heads.values()))
 
     def _heads_act(self, data_dict, m, extras, out=None):
-        f = crop_camera(self, encode(self, data_dict, m), m, extras)
+        f, crop = self._agent_feature(data_dict, m, extras)
+        if crop is not None:
+            f = center_crop_nhwc(f, *crop)
         # layer0 of layers_{m} never runs: the backbone's output is the first scale (heter_model_late.py:91-98)
         layers = getattr(self, f"layers_{m}")
         feats = [f]

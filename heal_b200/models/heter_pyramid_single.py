@@ -11,38 +11,26 @@ from .sub_modules.base_bev_backbone_resnet import ResNetBEVBackbone
 from .sub_modules.feature_alignnet import AlignNet
 from .sub_modules.downsample_conv import DownsampleConv
 from .fuse_modules.pyramid_fuse import PyramidFusion
-from .heter_pyramid_collab import FusedHeads
-from .heter_model_late import LateForward, build_encoder, crop_camera, encode
+from .heter_common import HeterFront, add_heads, center_crop_nhwc, modality_names
+from .heter_model_late import LateForward
 
 
-class HeterPyramidSingle(LateForward, nn.Module):
+class HeterPyramidSingle(LateForward, HeterFront, nn.Module):
+    adapter_name = "aligner"
+
     def __init__(self, args):
         super().__init__()
-        self.modality_name_list = [x for x in args.keys() if x.startswith("m") and x[1:].isdigit()]
+        self.modality_name_list = modality_names(args)
         self.cav_range = args['lidar_range']
         self.sensor_type_dict = OrderedDict()
         for m in self.modality_name_list:
             setting = args[m]
-            self.sensor_type_dict[m] = setting['sensor_type']
-            setattr(self, f"encoder_{m}", build_encoder(setting))
-            setattr(self, f"depth_supervision_{m}", bool(setting['encoder_args'].get("depth_supervision", False)))
-            setattr(self, f"backbone_{m}", ResNetBEVBackbone(setting['backbone_args']))
-            if setting['sensor_type'] == "camera":
-                g = setting['camera_mask_args']['grid_conf']
-                setattr(self, f"crop_ratio_W_{m}", self.cav_range[3] / g['xbound'][1])
-                setattr(self, f"crop_ratio_H_{m}", self.cav_range[4] / g['ybound'][1])
-            setattr(self, f"aligner_{m}", AlignNet(setting['aligner_args']))
+            self._add_modality(m, setting, ResNetBEVBackbone(setting['backbone_args']), AlignNet(setting['aligner_args']))
         self.pyramid_backbone = PyramidFusion(args['fusion_backbone'])
         self.shrink_flag = 'shrink_header' in args
         if self.shrink_flag:
             self.shrink_conv = DownsampleConv(args['shrink_header'])
-        self.cls_head = nn.Conv2d(args['in_head'], args['anchor_number'], kernel_size=1)
-        self.reg_head = nn.Conv2d(args['in_head'], 7 * args['anchor_number'], kernel_size=1)
-        self.dir_head = nn.Conv2d(args['in_head'], args['dir_args']['num_bins'] * args['anchor_number'], kernel_size=1)
-        self._heads = FusedHeads([self.cls_head, self.reg_head, self.dir_head])
-
-    def model_train_init(self):
-        pass
+        self._heads = add_heads(self, args['in_head'], args)
 
     def _any_heads(self):
         return self._heads
@@ -51,8 +39,9 @@ class HeterPyramidSingle(LateForward, nn.Module):
         return {'pyramid': 'single'}
 
     def _heads_act(self, data_dict, m, extras, out=None):
-        f = getattr(self, f"aligner_{m}").forward_nhwc(encode(self, data_dict, m))   # the aligner runs before the crop here
-        f = crop_camera(self, f, m, extras)
+        f, crop = self._agent_feature(data_dict, m, extras)       # the aligner runs before the crop here
+        if crop is not None:
+            f = center_crop_nhwc(f, *crop)
         pb = self.pyramid_backbone
         feats = pb.multiscale_nhwc(f)
         extras['occ_single_list'] = [ops.act_to_nchw(pb._occ_nhwc(x, i)) for i, x in enumerate(feats)]

@@ -11,7 +11,7 @@ from .sub_modules.point_pillar_scatter import PointPillarScatter
 from .sub_modules.base_bev_backbone import BaseBEVBackbone
 from .sub_modules.base_bev_backbone_resnet import ResNetBEVBackbone
 from .sub_modules.downsample_conv import DownsampleConv
-from .heter_pyramid_collab import FusedHeads
+from .heter_common import add_heads
 
 
 class PointPillar(nn.Module):
@@ -33,14 +33,8 @@ class PointPillar(nn.Module):
             self.out_channel = args['shrink_header']['dim'][-1]
         else:
             self.out_channel = sum(args['base_bev_backbone']['num_upsample_filter'])
-        self.cls_head = nn.Conv2d(self.out_channel, args['anchor_number'], kernel_size=1)
-        self.reg_head = nn.Conv2d(self.out_channel, 7 * args['anchor_number'], kernel_size=1)
         self.use_dir = 'dir_args' in args
-        heads = [self.cls_head, self.reg_head]
-        if self.use_dir:
-            self.dir_head = nn.Conv2d(self.out_channel, args['dir_args']['num_bins'] * args['anchor_number'], kernel_size=1)
-            heads.append(self.dir_head)
-        self._heads = FusedHeads(heads)
+        self._heads = add_heads(self, self.out_channel, args, use_dir=self.use_dir)
 
     def forward(self, data_dict):
         require_eval(self)

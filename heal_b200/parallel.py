@@ -107,16 +107,14 @@ def forward_agent_sharded(model, data_dict, rank: int, world: int):
     if offs_host is None:
         offs_host = inp['agent_offsets'].cpu().tolist()           # one-time host copy when the caller did not provide it
     pb = model.pyramid_backbone
-    enc, bb = getattr(model, f"encoder_{m}"), getattr(model, f"backbone_{m}")
     fmt = act_fmt()
-    # ---- local agents: encoder -> backbone -> ResNeXt levels + occ heads --------------------------------
+    # ---- local agents: encoder -> backbone -> aligner -> ResNeXt levels + occ heads ---------------------
     idle = len(mine) == 0
     use = mine if not idle else [0]                                # an idle rank computes agent 0 and discards it
     lo, hi = offs_host[use[0]], offs_host[use[-1] + 1]
     sub_offs = torch.tensor([o - lo for o in offs_host[use[0]:use[-1] + 2]], dtype=torch.int32, device=inp['points'].device)
     sub = {f'inputs_{m}': {'points': inp['points'][lo:hi], 'agent_offsets': sub_offs}}
-    x = enc.forward_act(sub, m)
-    x = bb.decode_nhwc(bb.multiscale_nhwc(x))
+    x = getattr(model, f"aligner_{m}").forward_nhwc(model._encode(sub, m))
     feats = pb.multiscale_nhwc(x)
     occs = [pb._occ_nhwc(f, i) for i, f in enumerate(feats)]
     def per_agent(a: "ops.Act"):
@@ -432,11 +430,8 @@ class AgentShardedFrame:
         pb = model.pyramid_backbone
         p2p = self.sym is not None
         side_i = sd["i"]
-        enc, bb = getattr(model, f"encoder_{m}"), getattr(model, f"backbone_{m}")
         sub = {f'inputs_{m}': {'points': self.points, 'agent_offsets': self.offsets}}
-        x = enc.forward_act(sub, m)
-        x = bb.decode_nhwc(bb.multiscale_nhwc(x))
-        x = getattr(model, f"aligner_{m}").forward_nhwc(x)
+        x = getattr(model, f"aligner_{m}").forward_nhwc(model._encode(sub, m))
         # ResNeXt levels: the last conv of each level writes into my chunk of the gather buffer; in p2p mode the level's block is
         # pushed to the peers on the side stream while the next level computes
         S = self.slots

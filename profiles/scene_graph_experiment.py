@@ -93,9 +93,9 @@ def timed(fn, iters):
 def legacy_stack(feats, aml, crops):
     """The agent assembly the forwards ran before heal_agent_stack: convert, CenterCrop with torch pad / slicing, torch.cat."""
     from heal_b200 import ops
-    from heal_b200.models.heter_pyramid_collab import HeterPyramidCollab
+    from heal_b200.models.heter_common import crop_tensor
     f32 = {m: ops.convert(f, "f32").t for m, f in feats.items()}
-    f32 = {m: HeterPyramidCollab._crop_tensor(f, *crops[m]) if m in crops else f for m, f in f32.items()}
+    f32 = {m: crop_tensor(f, *crops[m]) if m in crops else f for m, f in f32.items()}
     cnt = {m: 0 for m in f32}
     rows = []
     for m in aml:
@@ -162,13 +162,9 @@ def main():
         feats, crops = {}, {}
         d = dev[0]
         for m in ("m1", "m2", "m3", "m4"):
-            enc = getattr(model, f"encoder_{m}")
-            f = enc.forward_act(d, m)
-            bb = getattr(model, f"backbone_{m}")
-            f = getattr(model, f"aligner_{m}").forward_nhwc(bb.decode_nhwc(bb.multiscale_nhwc(f)))
-            if model.sensor_type_dict[m] == "camera":
-                crops[m] = (int(f.H * getattr(model, f"crop_ratio_H_{m}")), int(f.W * getattr(model, f"crop_ratio_W_{m}")))
-            feats[m] = f
+            feats[m], crop = model._agent_feature(d, m, {})
+            if crop is not None:
+                crops[m] = crop
         assert torch.equal(ops.agent_stack(feats, AML, crops).t, legacy_stack(feats, AML, crops).t)
         arms = {"eager": lambda n: timed(eager, n), "scene_graph": lambda n: timed(replay, n),
                 "pipeline_boxes": piped(pipes["boxes"]), "pipeline_heads": piped(pipes["heads"]),
