@@ -77,6 +77,7 @@ SIGNATURES = {
                                       _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "heal_eval_workspace": (_sz, [_i, _i]),
     "heal_eval_tp_fp": (_i, [_vp, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "heal_eval_tp_fp_counted": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "heal_spconv_table_size": (_sz, [_i]),
     "heal_spconv_build_table": (_i, [_vp, _vp, _i, _vp, _i, _vp, _vp, _vp]),
     "heal_spconv_subm_neighbors": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp]),

@@ -11,6 +11,11 @@
 //   k_match  one warp per threshold, all thresholds at once: the greedy pass in score order (eval_utils.py:74-87).  Each det
 //            reduces the max IoU and its first argmax over the GTs not yet taken; it is a TP unless no GT remains or max < thr in
 //            fp32 (NumPy 2 casts the Python threshold to the array's float32), and a TP takes its argmax GT.
+// Two entry points share these kernels.  heal_eval_tp_fp takes K and G from the host and sizes everything by them.
+// heal_eval_tp_fp_counted reads K and G from device ints (e.g. the box count heal_box_decode_nms writes), so it can follow the
+// post-processing in one captured graph: grids, workspace and output strides follow host capacities, every kernel reads the
+// live counts and leaves the rows and columns beyond them alone, and a count above its capacity sets HEAL_EVAL_OVER_CAPACITY
+// (k_polys) and makes every kernel return.
 #include "common.cuh"
 #include "quad_iou.cuh"
 #include "../../include/heal_b200.h"
@@ -22,11 +27,28 @@ constexpr int kMaxThr = 8;
 
 struct Thresholds { float v[kMaxThr]; };
 
-// poly rows: 8 doubles (ccw x0 y0 .. x3 y3) + area; rows 0..K-1 the dets, K..K+G-1 the GTs
-__global__ void k_polys(const float* __restrict__ det, int K, const float* __restrict__ gt, int G, double* __restrict__ poly) {
+// The frame's sizes.  k_dev / g_dev NULL: the live counts are k / g (== kcap / gcap).  Else the live counts are *k_dev / *g_dev,
+// read on the device, and kcap / gcap size the grids, the poly rows and the strides of the IoU matrix and of the flags.
+struct Counts { const int* k_dev; const int* g_dev; int k, g, kcap, gcap; };
+
+// the live (K, G); false when a device count lies outside [0, capacity] (nothing is then computed)
+__device__ __forceinline__ bool live(const Counts& c, int& K, int& G) {
+    K = c.k_dev ? __ldg(c.k_dev) : c.k;
+    G = c.g_dev ? __ldg(c.g_dev) : c.g;
+    return K >= 0 && K <= c.kcap && G >= 0 && G <= c.gcap;
+}
+
+// poly rows: 8 doubles (ccw x0 y0 .. x3 y3) + area; rows 0..kcap-1 the dets, kcap..kcap+gcap-1 the GTs
+__global__ void k_polys(const float* __restrict__ det, const float* __restrict__ gt, Counts c, double* __restrict__ poly,
+                        int* __restrict__ status) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= K + G) return;
-    quad_ccw(i < K ? det + (size_t)i * 24 : gt + (size_t)(i - K) * 24, poly + (size_t)i * 9);
+    int K, G;
+    if (!live(c, K, G)) {
+        if (i == 0) atomicOr(status, HEAL_EVAL_OVER_CAPACITY);
+        return;
+    }
+    if (i < c.kcap ? i >= K : i - c.kcap >= G) return;
+    quad_ccw(i < c.kcap ? det + (size_t)i * 24 : gt + (size_t)(i - c.kcap) * 24, poly + (size_t)i * 9);
 }
 
 // a ranks before b: descending score, NaN last, ties by ascending index
@@ -37,8 +59,10 @@ __device__ __forceinline__ bool ranks_before(float a, int ia, float b, int ib) {
 }
 
 __global__ void __launch_bounds__(256)
-k_rank(const float* __restrict__ scores, int K, int* __restrict__ perm, float* __restrict__ sorted_scores) {
+k_rank(const float* __restrict__ scores, Counts c, int* __restrict__ perm, float* __restrict__ sorted_scores) {
     __shared__ float ss[1024];
+    int K, G;
+    if (!live(c, K, G)) return;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const float s = i < K ? scores[i] : 0.f;
     int rank = 0;
@@ -53,27 +77,31 @@ k_rank(const float* __restrict__ scores, int K, int* __restrict__ perm, float* _
     if (i < K) { perm[rank] = i; sorted_scores[rank] = s; }
 }
 
-// row r of iou = sorted det r against every GT
+// row r of iou (stride gcap) = sorted det r against every GT
 __global__ void __launch_bounds__(128)
-k_iou(const double* __restrict__ poly, const int* __restrict__ perm, int K, int G, float* __restrict__ iou, int* __restrict__ status) {
+k_iou(const double* __restrict__ poly, const int* __restrict__ perm, Counts c, float* __restrict__ iou, int* __restrict__ status) {
+    int K, G;
+    if (!live(c, K, G)) return;
     const int r = blockIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= G) return;
+    if (r >= K || j >= G) return;
     double P[9], Q[9];
     const double* p = poly + (size_t)perm[r] * 9;
-    const double* q = poly + (size_t)(K + j) * 9;
+    const double* q = poly + (size_t)(c.kcap + j) * 9;
 #pragma unroll
     for (int k = 0; k < 9; ++k) { P[k] = p[k]; Q[k] = q[k]; }
     const double inter = quad_bbox_disjoint(P, Q) ? 0.0 : quad_intersection(P, Q);
     const double uni = P[8] + Q[8] - inter;           // QuadPolygon.union: self.area + o.area - intersection, self = the det
     if (uni == 0.0) atomicOr(status, HEAL_EVAL_ZERO_UNION);
-    iou[(size_t)r * G + j] = (float)(inter / uni);
+    iou[(size_t)r * c.gcap + j] = (float)(inter / uni);
 }
 
 // one warp per threshold (blockIdx.x); `taken` marks the GTs matched so far.  NaN IoUs (zero unions, reported in the status word)
-// never win the max.
+// never win the max.  Flags of threshold t at tp[t * kcap ..].
 __global__ void __launch_bounds__(32)
-k_match(const float* __restrict__ iou, int K, int G, Thresholds thr, unsigned char* __restrict__ tp) {
+k_match(const float* __restrict__ iou, Counts c, Thresholds thr, unsigned char* __restrict__ tp) {
     __shared__ unsigned char taken[kMaxBoxes];
+    int K, G;
+    if (!live(c, K, G)) return;
     const int t = blockIdx.x, lane = threadIdx.x;
     for (int j = lane; j < G; j += 32) taken[j] = 0;
     __syncwarp();
@@ -82,7 +110,7 @@ k_match(const float* __restrict__ iou, int K, int G, Thresholds thr, unsigned ch
     for (int r = 0; r < K; ++r) {
         unsigned char flag = 0;
         if (left > 0) {
-            const float* row = iou + (size_t)r * G;
+            const float* row = iou + (size_t)r * c.gcap;
             float best = -INFINITY;
             int arg = 0x7fffffff;
 #pragma unroll 4
@@ -103,7 +131,7 @@ k_match(const float* __restrict__ iou, int K, int G, Thresholds thr, unsigned ch
             }
             __syncwarp();
         }
-        if (lane == 0) tp[(size_t)t * K + r] = flag;
+        if (lane == 0) tp[(size_t)t * c.kcap + r] = flag;
     }
 }
 
@@ -120,6 +148,32 @@ WsLayout layout(int K, int G) {
     return L;
 }
 
+// the thresholds of a call -> the kernel argument; false for a count outside [1, 8] or a threshold that is not > 0 (NaN included)
+bool thresholds(const float* thresholds_host, int n_thr, Thresholds& thr) {
+    if (n_thr < 1 || n_thr > kMaxThr || !thresholds_host) return false;
+    for (int t = 0; t < kMaxThr; ++t) thr.v[t] = 0.f;
+    for (int t = 0; t < n_thr; ++t) {
+        if (!(thresholds_host[t] > 0.f)) return false;
+        thr.v[t] = thresholds_host[t];
+    }
+    return true;
+}
+
+// the kernels over kcap >= 1 dets and gcap GTs (k_iou only when gcap > 0); status_out cleared first
+int launch(const float* det_corners, const float* det_scores, const float* gt_corners, const Counts& c, const Thresholds& thr,
+           int n_thr, float* sorted_scores_out, unsigned char* tp_out, int* status_out, void* ws, cudaStream_t st) {
+    const WsLayout L = layout(c.kcap, c.gcap);
+    uint8_t* w = (uint8_t*)ws;
+    double* poly = (double*)(w + L.poly);
+    int* perm = (int*)(w + L.perm);
+    float* iou = (float*)(w + L.iou);
+    k_polys<<<(c.kcap + c.gcap + 127) / 128, 128, 0, st>>>(det_corners, gt_corners, c, poly, status_out);
+    k_rank<<<(c.kcap + 255) / 256, 256, 0, st>>>(det_scores, c, perm, sorted_scores_out);
+    if (c.gcap > 0) k_iou<<<dim3((c.gcap + 127) / 128, c.kcap), 128, 0, st>>>(poly, perm, c, iou, status_out);
+    k_match<<<n_thr, 32, 0, st>>>(iou, c, thr, tp_out);
+    return heal_check_launch(c.gcap > 0 ? 4 : 3);
+}
+
 }  // namespace
 
 extern "C" size_t heal_eval_workspace(int K, int G) {
@@ -130,28 +184,31 @@ extern "C" size_t heal_eval_workspace(int K, int G) {
 extern "C" int heal_eval_tp_fp(const float* det_corners, const float* det_scores, int K, const float* gt_corners, int G,
                                const float* thresholds_host, int n_thr, float* sorted_scores_out, unsigned char* tp_out,
                                int* status_out, void* ws, size_t ws_bytes, void* stream_) {
-    if (K < 0 || K > kMaxBoxes || G < 0 || G > kMaxBoxes || n_thr < 1 || n_thr > kMaxThr || !thresholds_host || !status_out)
-        return HEAL_ERR_ARG;
     Thresholds thr;
-    for (int t = 0; t < kMaxThr; ++t) thr.v[t] = 0.f;
-    for (int t = 0; t < n_thr; ++t) {
-        if (!(thresholds_host[t] > 0.f)) return HEAL_ERR_ARG;             // also rejects NaN
-        thr.v[t] = thresholds_host[t];
-    }
+    if (K < 0 || K > kMaxBoxes || G < 0 || G > kMaxBoxes || !thresholds(thresholds_host, n_thr, thr) || !status_out)
+        return HEAL_ERR_ARG;
     if (K > 0 && (!det_corners || !det_scores || !sorted_scores_out || !tp_out)) return HEAL_ERR_ARG;
     if (G > 0 && !gt_corners) return HEAL_ERR_ARG;
-    const WsLayout L = layout(K, G);
-    if (!ws || ws_bytes < L.total) return HEAL_ERR_ARG;
+    if (!ws || ws_bytes < layout(K, G).total) return HEAL_ERR_ARG;
     cudaStream_t st = (cudaStream_t)stream_;
     if (cudaMemsetAsync(status_out, 0, sizeof(int), st) != cudaSuccess) return HEAL_ERR_LAUNCH;
     if (K == 0) return HEAL_OK;
-    uint8_t* w = (uint8_t*)ws;
-    double* poly = (double*)(w + L.poly);
-    int* perm = (int*)(w + L.perm);
-    float* iou = (float*)(w + L.iou);
-    k_polys<<<(K + G + 127) / 128, 128, 0, st>>>(det_corners, K, gt_corners, G, poly);
-    k_rank<<<(K + 255) / 256, 256, 0, st>>>(det_scores, K, perm, sorted_scores_out);
-    if (G > 0) k_iou<<<dim3((G + 127) / 128, K), 128, 0, st>>>(poly, perm, K, G, iou, status_out);
-    k_match<<<n_thr, 32, 0, st>>>(iou, K, G, thr, tp_out);
-    return heal_check_launch(G > 0 ? 4 : 3);
+    const Counts c{nullptr, nullptr, K, G, K, G};
+    return launch(det_corners, det_scores, gt_corners, c, thr, n_thr, sorted_scores_out, tp_out, status_out, ws, st);
+}
+
+extern "C" int heal_eval_tp_fp_counted(const float* det_corners, const float* det_scores, const int* det_count, int K_cap,
+                                       const float* gt_corners, const int* gt_count, int G_cap, const float* thresholds_host,
+                                       int n_thr, float* sorted_scores_out, unsigned char* tp_out, int* status_out, void* ws,
+                                       size_t ws_bytes, void* stream_) {
+    Thresholds thr;
+    if (K_cap < 1 || K_cap > kMaxBoxes || G_cap < 1 || G_cap > kMaxBoxes || !thresholds(thresholds_host, n_thr, thr))
+        return HEAL_ERR_ARG;
+    if (!det_corners || !det_scores || !det_count || !gt_corners || !gt_count || !sorted_scores_out || !tp_out || !status_out)
+        return HEAL_ERR_ARG;
+    if (!ws || ws_bytes < layout(K_cap, G_cap).total) return HEAL_ERR_ARG;
+    cudaStream_t st = (cudaStream_t)stream_;
+    if (cudaMemsetAsync(status_out, 0, sizeof(int), st) != cudaSuccess) return HEAL_ERR_LAUNCH;
+    const Counts c{det_count, gt_count, 0, 0, K_cap, G_cap};
+    return launch(det_corners, det_scores, gt_corners, c, thr, n_thr, sorted_scores_out, tp_out, status_out, ws, st);
 }

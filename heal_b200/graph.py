@@ -114,7 +114,8 @@ class FrameInterleaver:
     @classmethod
     def for_scene(cls, model, agent_modality_list, capacities, pairwise_shape, postprocess_params=None, n: int = 2,
                   device=None, **graph_kwargs):
-        """N captured SceneGraphs of a mixed-modality scene; `submit(ego_batch)` loads and replays one."""
+        """N captured SceneGraphs of a mixed-modality scene; `submit(ego_batch)` (`submit(ego_batch, gt_boxes)` with
+        `eval_thresholds`) loads and replays one."""
         dev = device or next(model.parameters()).device
         il = SceneInterleaver.__new__(SceneInterleaver)
         il._start([SceneGraph(model, agent_modality_list, capacities, pairwise_shape, postprocess_params, device=dev,
@@ -179,21 +180,29 @@ class FramePipeline:
 
     @classmethod
     def for_scene(cls, model, agent_modality_list, capacities, pairwise_shape, postprocess_params=None, device=None,
-                  compute_streams: int = 2, depth: int = 2, **graph_kwargs):
+                  compute_streams: int = 2, depth: int = 2, eval_thresholds=None, gt_capacity=None, **graph_kwargs):
         """The pipeline over a mixed-modality scene (SceneGraph slots): `submit(ego_batch)` takes the reference's collated
         `batch_data['ego']` and returns, pinned on the host, the boxes, scores and box count of frame i - (depth - 1) when
-        `postprocess_params` is given (`boxes[:count[0]]`), else its heads."""
+        `postprocess_params` is given (`boxes[:count[0]]`), else its heads.  With `eval_thresholds` (and `gt_capacity`, see
+        SceneGraph) `submit(ego_batch, gt_boxes)` also takes the frame's GT, each frame is evaluated in its graph, and
+        `pipe.result_stat` collects the frames in the reference's format as they come back."""
         dev = device or next(model.parameters()).device
-        graphs = [SceneGraph(model, agent_modality_list, capacities, pairwise_shape, postprocess_params, device=dev, **graph_kwargs)
+        graphs = [SceneGraph(model, agent_modality_list, capacities, pairwise_shape, postprocess_params, device=dev,
+                             eval_thresholds=eval_thresholds, gt_capacity=gt_capacity, **graph_kwargs)
                   for _ in range(max(2, int(depth)))]
         pipe = ScenePipeline.__new__(ScenePipeline)
-        pipe._start(graphs, [g.results() for g in graphs], dev, compute_streams)
+        pipe._start(graphs, [g.results() for g in graphs], dev, compute_streams, graphs[0].eval_thresholds)
         return pipe
 
-    def _start(self, graphs, results, dev, compute_streams):
+    def _start(self, graphs, results, dev, compute_streams, eval_thresholds=None):
         """`results[k]`: the device tensors slot k copies back to the host after each replay, by name (None: bound later by
-        `_bind`, when the slot's first graph exists)."""
+        `_bind`, when the slot's first graph exists).  With `eval_thresholds` the results carry each frame's evaluation
+        (SceneGraph.results), which goes into `result_stat` as the frame is handed back."""
         self.dev, self.depth = dev, len(graphs)
+        self.eval_thresholds = eval_thresholds
+        self.result_stat = None if eval_thresholds is None else \
+            {t: {'tp': [], 'fp': [], 'score': [], 'gt': 0} for t in eval_thresholds}
+        self.evaluated = 0                                     # frames appended to result_stat (or refused by it) so far
         self.graphs = graphs
         self.s_in, self.s_out = (torch.cuda.Stream(device=dev) for _ in range(2))
         comp = [torch.cuda.Stream(device=dev) for _ in range(2 if compute_streams >= 2 else 1)]
@@ -227,6 +236,17 @@ class FramePipeline:
         """What `submit` / `drain` hand back for the frame that last used slot k."""
         return self.host_out[k]
 
+    def _returned(self, c):
+        """The result of frame c (complete on the host).  With evaluation, the first time frame c is handed back its flags go
+        into `result_stat`, in frame order; a frame whose evaluation failed raises here and is not appended again."""
+        r = self._result(c % self.depth)
+        if self.result_stat is not None and c >= self.evaluated:
+            from .utils.eval_utils import append_packed
+            self.evaluated = c + 1
+            append_packed(self.result_stat, self.eval_thresholds, r["eval"], int(r["count"][0]), r["scores"].shape[0],
+                          int(r["gt_count"][0]))
+        return r
+
     def submit(self, points: torch.Tensor, offsets: torch.Tensor, pairwise: torch.Tensor):
         return self._submit(points, offsets, pairwise)
 
@@ -234,7 +254,6 @@ class FramePipeline:
         d = self.depth
         k = self.count % d
         g = self._slot(k, *inputs)
-        prev = None
         with torch.cuda.stream(self.s_in):
             if self.count >= d:
                 self.s_in.wait_event(self.ev_comp[k])          # frame count-depth has consumed these input buffers
@@ -252,20 +271,19 @@ class FramePipeline:
             for name, h in self.host_out[k].items():
                 h.copy_(self.dev_out[k][name], non_blocking=True)
             self.ev_out[k].record(self.s_out)
-        if self.count >= d - 1:
-            j = (self.count - (d - 1)) % d
-            self.ev_out[j].synchronize()                       # frame count-(depth-1) is complete on the host
-            prev = self._result(j)
+        frame = self.count - (d - 1)
+        if frame >= 0:
+            self.ev_out[frame % d].synchronize()               # frame count-(depth-1) is complete on the host
         self.h2d_bytes = h2d
         self.count += 1
-        return prev
+        return self._returned(frame) if frame >= 0 else None
 
     def drain(self):
         """Predictions of the frames still in flight, oldest first (the results `submit` has not returned yet)."""
         out = []
         for c in range(max(self.count - (self.depth - 1), 0), self.count):
             self.ev_out[c % self.depth].synchronize()
-            out.append(self._result(c % self.depth))
+            out.append(self._returned(c))
         return out
 
     def flush(self):
@@ -371,6 +389,71 @@ def _anchor_box(postprocess_params):
     return VoxelPostprocessor(postprocess_params, False).generate_anchor_box()
 
 
+def eval_setup(postprocess_params, eval_thresholds, gt_capacity):
+    """(thresholds, GT capacity) of a captured frame that evaluates its boxes, or (None, None) when `eval_thresholds` is None.
+    Checked on the host: evaluation needs `postprocess_params`; 1 to 8 thresholds, each > 0; the GT capacity is `gt_capacity`,
+    by default `postprocess_params['max_num']` (100 in the shipped yamls), and lies in [1, 4096].  Raises ValueError."""
+    if eval_thresholds is None:
+        if gt_capacity is not None:
+            raise ValueError("gt_capacity without eval_thresholds: the frame does not evaluate its boxes")
+        return None, None
+    if postprocess_params is None:
+        raise ValueError("evaluation matches the post-processed boxes: eval_thresholds needs postprocess_params")
+    thr = tuple(float(v) for v in eval_thresholds)
+    if not 1 <= len(thr) <= 8 or not all(v > 0 for v in thr):
+        raise ValueError(f"eval_thresholds {eval_thresholds}: 1 to 8 IoU thresholds, each > 0")
+    if gt_capacity is None:
+        if 'max_num' not in postprocess_params:
+            raise ValueError("gt_capacity: postprocess_params has no 'max_num'; give the most GT boxes a frame may have")
+        gt_capacity = postprocess_params['max_num']
+    if not _count(gt_capacity) or gt_capacity > 4096:
+        raise ValueError(f"gt_capacity {gt_capacity!r}: an int in [1, 4096]")
+    return thr, int(gt_capacity)
+
+
+def check_gt(gt_boxes, gt_capacity):
+    """Host-side checks of a frame's GT against a captured frame's GT capacity (None: the frame does not evaluate): GT
+    (G, 8, 3) fp32 corners, as the reference's post_processor.generate_gt_bbx returns them, with G <= capacity, required when the
+    frame evaluates and refused when it does not.  Raises ValueError; returns the bytes the load copies."""
+    if gt_capacity is None:
+        if gt_boxes is not None:
+            raise ValueError("gt_boxes given to a frame captured without eval_thresholds")
+        return 0
+    if gt_boxes is None:
+        raise ValueError("the frame evaluates its boxes (eval_thresholds): gt_boxes (G, 8, 3) fp32 required")
+    if not isinstance(gt_boxes, torch.Tensor) or gt_boxes.dim() != 3 or tuple(gt_boxes.shape[1:]) != (8, 3):
+        raise ValueError(f"gt_boxes of shape {tuple(getattr(gt_boxes, 'shape', ()))}, (G, 8, 3) corners expected")
+    if gt_boxes.dtype != torch.float32:
+        raise ValueError(f"gt_boxes of dtype {gt_boxes.dtype}, float32 corners expected")
+    if gt_boxes.shape[0] > gt_capacity:
+        raise ValueError(f"the frame has {gt_boxes.shape[0]} GT boxes, the graph's gt_capacity is {gt_capacity}")
+    return gt_boxes.shape[0] * 96 + 4
+
+
+class FrameEval:
+    """The evaluation of a captured frame: its static GT input (`gt` (capacity, 8, 3) fp32 corners, `gt_count` (1,) int32) and
+    the ops.EvalBuffers heal_eval_tp_fp_counted writes, for up to `det_capacity` boxes (the post-processing's `top`).  Caller-owned
+    so that several graphs can share one (SceneStream: one per pipeline slot, outside the graph pool)."""
+
+    def __init__(self, det_capacity: int, gt_capacity: int, device):
+        from . import ops
+        self.gt = torch.zeros((gt_capacity, 8, 3), dtype=torch.float32, device=device)
+        self.gt_count = torch.zeros((1,), dtype=torch.int32, device=device)
+        self.buffers = ops.EvalBuffers(det_capacity, gt_capacity, device)
+
+    def run(self, post, thresholds):
+        """Match the post-processed boxes (ops.PostprocessBuffers: boxes, scores, count on the device) to the GT; capture-safe."""
+        from . import ops
+        return ops.eval_tp_fp_counted(post.boxes, post.scores, post.count, self.gt, self.gt_count, thresholds, self.buffers)
+
+    def load(self, gt_boxes):
+        """Copy a frame's GT (checked by check_gt) into the static buffers, asynchronously on the current stream."""
+        n = gt_boxes.shape[0]
+        if n:
+            self.gt[:n].copy_(gt_boxes, non_blocking=True)
+        self.gt_count.fill_(n)
+
+
 class LateFusionGraph:
     """Late fusion of one scene as ONE captured graph: a single-agent model's `grouped_heads` (one batched forward per modality,
     every cav's heads in one (n_cav, H, W, S) buffer) and heal_box_decode_nms_late (decode with the transforms read on the device,
@@ -380,6 +463,11 @@ class LateFusionGraph:
         g.load(batch_data)            # {cav_id: {inputs_<m>: ..., transformation_matrix: 4x4}} in the captured modality order
         out = g.replay()              # out.boxes[:out.count], out.scores[:out.count] on the device, no host sync
 
+    With `eval_thresholds` (e.g. inference.py's (0.3, 0.5, 0.7)) the graph ends in heal_eval_tp_fp_counted, which matches the
+    boxes to the GT given to `load(batch_data, gt_boxes)`: `g.eval.buffers.packed` holds the frame's status, sorted scores and
+    flags at the capacity `top` (eval_utils.append_packed turns a host copy into `result_stat` entries).  Late fusion's GT is the
+    union of every cav's objects, so `gt_capacity` (default `postprocess_params['max_num']`) may need to be larger than an
+    intermediate-fusion frame's.
     `capacities[m]`: for a lidar modality the point capacity of ALL its cavs together (raw clouds, `points` + `agent_offsets`; the
     live counts travel in the offsets), for a camera modality (cameras, image height, image width) per cav for normalised fp32
     images, or (cameras, frame height, frame width, torch.uint8) for raw uint8 (H0, W0, 3) frames, which the encoder resizes, crops
@@ -387,10 +475,13 @@ class LateFusionGraph:
 
     CAMERA_KEYS = ("rots", "trans", "intrins", "post_rots", "post_trans")
 
-    def __init__(self, model, modality_of_each_cav, capacities, postprocess_params, device=None, warmup: int = 2, top: int = 1000):
+    def __init__(self, model, modality_of_each_cav, capacities, postprocess_params, device=None, warmup: int = 2, top: int = 1000,
+                 eval_thresholds=None, gt_capacity=None):
         from . import ops
         from .data_utils.post_processor.voxel_postprocessor import VoxelPostprocessor
         dev = device or next(model.parameters()).device
+        self.eval_thresholds, self.gt_capacity = eval_setup(postprocess_params, eval_thresholds, gt_capacity)
+        self.eval = FrameEval(top, self.gt_capacity, dev) if self.eval_thresholds is not None else None
         self.modalities = list(modality_of_each_cav)
         n = len(self.modalities)
         self.groups = {}
@@ -407,11 +498,14 @@ class LateFusionGraph:
 
         def run():
             y, _ = model.grouped_heads(self.groups, self.inputs, n)
-            return ops.box_decode_nms_late(y, y, y, self.anchors, self.transforms,
+            post = ops.box_decode_nms_late(y, y, y, self.anchors, self.transforms,
                                            postprocess_params['target_args']['score_threshold'], postprocess_params['nms_thresh'],
                                            dir_offset=dargs.get('dir_offset', 0.0), num_bins=bins, order=postprocess_params['order'],
                                            gt_range=postprocess_params['gt_range'], top=top, buffers=self.buffers,
                                            coffsets=(0, A, 8 * A))
+            if self.eval is not None:
+                self.eval.run(post, self.eval_thresholds)
+            return post
 
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
@@ -426,14 +520,16 @@ class LateFusionGraph:
             self.out = run()
         self.kernels_per_replay = int(lib.heal_launch_count() - l0)
 
-    def load(self, batch_data):
+    def load(self, batch_data, gt_boxes=None):
         """Copy a scene's inputs and cav -> ego transforms into the captured buffers (asynchronous copies on the current stream).
-        The cavs must come in the captured modality order; each lidar cav carries one raw cloud (`points`, `agent_offsets`)."""
+        The cavs must come in the captured modality order; each lidar cav carries one raw cloud (`points`, `agent_offsets`).
+        `gt_boxes`: the scene's GT corners (G, 8, 3) fp32, required with evaluation and refused without (check_gt)."""
         from .models.heter_model_late import modality_of
         cavs = list(batch_data.keys())
         mods = [modality_of(batch_data[c]) for c in cavs]
         if mods != self.modalities:
             raise ValueError(f"scene modalities {mods}, the graph was captured for {self.modalities}")
+        check_gt(gt_boxes, self.gt_capacity)
         for m, idx in self.groups.items():
             buf = self.inputs[m]
             if "points" in buf:
@@ -454,20 +550,23 @@ class LateFusionGraph:
                         buf[k][j].copy_(src[k][0][:, :3] if k == "imgs" and not raw else src[k][0], non_blocking=True)
         T = torch.stack([torch.as_tensor(batch_data[c]['transformation_matrix']).reshape(4, 4).to(torch.float32) for c in cavs])
         self.transforms.copy_(T, non_blocking=True)
+        if self.eval is not None:
+            self.eval.load(gt_boxes)
 
     def replay(self):
         self.graph.replay()
         return self.out
 
 
-def check_scene(spec, agent_modality_list, voxel_limits, ego_batch):
+def check_scene(spec, agent_modality_list, voxel_limits, ego_batch, gt_boxes=None, gt_capacity=None):
     """Host-side checks of a collated `batch_data['ego']` against a captured scene (no device read): the agent modalities, every
-    input's shape against its buffer, the lidar voxelisation limits the graph was captured with, and uint8 frames against fp32
-    images.  Raises ValueError; returns the bytes `SceneGraph.load` copies."""
+    input's shape against its buffer, the lidar voxelisation limits the graph was captured with, uint8 frames against fp32
+    images, and the frame's GT against the graph's `gt_capacity` (check_gt; None: the graph does not evaluate).  Raises
+    ValueError; returns the bytes `SceneGraph.load` copies."""
     aml = list(ego_batch["agent_modality_list"])
     if aml != list(agent_modality_list):
         raise ValueError(f"scene modalities {aml}, the graph was captured for {list(agent_modality_list)}")
-    nbytes = ego_batch["pairwise_t_matrix"].numel() * 8
+    nbytes = ego_batch["pairwise_t_matrix"].numel() * 8 + check_gt(gt_boxes, gt_capacity)
     for m, sp in spec.items():
         src = ego_batch[f"inputs_{m}"]
         k = sp["agents"]
@@ -523,14 +622,23 @@ class SceneGraph:
 
     Several graphs can share memory (SceneStream does so per pipeline slot): `inputs` are caller-owned input buffers, as
     `_input_buffers` makes them for these capacities and as many or more agents (the graph reads leading slices);
-    `postprocess_buffers` are caller-owned ops.PostprocessBuffers for the box decode; `pool` is the private memory pool the frame
-    is captured into (torch.cuda.graph_pool_handle()).  The warm-up frames run outside the pool, so weight caches built lazily
-    land in the ordinary allocator."""
+    `postprocess_buffers` are caller-owned ops.PostprocessBuffers for the box decode; `eval_buffers` a caller-owned FrameEval;
+    `pool` is the private memory pool the frame is captured into (torch.cuda.graph_pool_handle()).  The warm-up frames run outside
+    the pool, so weight caches built lazily land in the ordinary allocator.
+
+    Evaluation: with `eval_thresholds` (inference.py's are (0.3, 0.5, 0.7)) the graph ends in heal_box_decode_nms ->
+    heal_eval_tp_fp_counted, which matches the ego's boxes to the frame's GT on the device (the box count never leaves it).  The
+    GT comes in with `load(ego_batch, gt_boxes)`: (G, 8, 3) fp32 corners, what the reference's
+    `post_processor.generate_gt_bbx(batch_data)` returns on the host, copied into a static (gt_capacity, 8, 3) buffer and a
+    device count.  `gt_capacity` defaults to `postprocess_params['max_num']` and must be given when that key is absent.
+    `results()` then adds the packed evaluation (ops.EvalBuffers: status, sorted scores, flags at capacity `top`) and G."""
 
     def __init__(self, model, agent_modality_list, capacities, pairwise_shape, postprocess_params=None, device=None,
-                 voxel_limits=None, warmup: int = 2, top: int = 1000, inputs=None, pool=None, postprocess_buffers=None):
+                 voxel_limits=None, warmup: int = 2, top: int = 1000, inputs=None, pool=None, postprocess_buffers=None,
+                 eval_thresholds=None, gt_capacity=None, eval_buffers=None):
         from . import ops
         dev = device or next(model.parameters()).device
+        self.eval_thresholds, self.gt_capacity = eval_setup(postprocess_params, eval_thresholds, gt_capacity)
         self.modalities = list(agent_modality_list)
         n = len(self.modalities)
         self.spec = scene_spec(model.sensor_type_dict, self.modalities, capacities)
@@ -546,6 +654,9 @@ class SceneGraph:
             self.anchors = torch.from_numpy(_anchor_box(postprocess_params)).to(device=dev, dtype=torch.float32).contiguous()
             H, W, A = self.anchors.shape[:3]
             self.postprocess = ops.PostprocessBuffers(H, W, A, top, dev) if postprocess_buffers is None else postprocess_buffers
+        self.eval = None
+        if self.eval_thresholds is not None:
+            self.eval = FrameEval(top, self.gt_capacity, dev) if eval_buffers is None else eval_buffers
         pparams, eye = postprocess_params, torch.eye(4, dtype=torch.float64)
 
         def run():
@@ -557,6 +668,8 @@ class SceneGraph:
                     pparams['target_args']['score_threshold'], pparams['nms_thresh'], dir_offset=dargs.get('dir_offset', 0.0),
                     num_bins=dargs.get('num_bins', 2), order=pparams['order'], gt_range=pparams['gt_range'], top=top,
                     buffers=self.postprocess)
+                if self.eval is not None:
+                    self.eval.run(out['postprocess'], self.eval_thresholds)
             return out
 
         side = torch.cuda.Stream(device=dev)
@@ -572,10 +685,11 @@ class SceneGraph:
             self.out = run()
         self.kernels_per_replay = int(lib.heal_launch_count() - l0)
 
-    def load(self, ego_batch):
-        """Copy a scene's inputs and pairwise transforms into the captured buffers (asynchronous copies on the current stream,
-        device or pinned-host sources).  Checks the batch on the host first (check_scene); returns the bytes copied."""
-        nbytes = check_scene(self.spec, self.modalities, self.voxel_limits, ego_batch)
+    def load(self, ego_batch, gt_boxes=None):
+        """Copy a scene's inputs and pairwise transforms (and with evaluation its GT corners) into the captured buffers
+        (asynchronous copies on the current stream, device or pinned-host sources).  Checks the batch on the host first
+        (check_scene); returns the bytes copied."""
+        nbytes = check_scene(self.spec, self.modalities, self.voxel_limits, ego_batch, gt_boxes, self.gt_capacity)
         for m, buf in self.inputs.items():
             src = ego_batch[f"inputs_{m}"]
             if "points" in buf:
@@ -588,6 +702,8 @@ class SceneGraph:
                 for k in LateFusionGraph.CAMERA_KEYS:
                     buf[k].copy_(src[k], non_blocking=True)
         self.pairwise.copy_(ego_batch["pairwise_t_matrix"], non_blocking=True)
+        if self.eval is not None:
+            self.eval.load(gt_boxes)
         return nbytes
 
     def replay(self):
@@ -596,24 +712,27 @@ class SceneGraph:
 
     def results(self):
         """The device tensors a frame's consumer reads: the ego's boxes, scores and box count with `postprocess_params`, else
-        the heads."""
+        the heads; with evaluation also `eval` (EvalBuffers.packed at capacity `top`) and `gt_count`."""
         if self.postprocess is not None:
-            return {"boxes": self.postprocess.boxes, "scores": self.postprocess.scores, "count": self.postprocess.count}
+            out = {"boxes": self.postprocess.boxes, "scores": self.postprocess.scores, "count": self.postprocess.count}
+            if self.eval is not None:
+                out.update(eval=self.eval.buffers.packed, gt_count=self.eval.gt_count)
+            return out
         return {k: self.out[k] for k in FramePipeline.OUT_KEYS if k in self.out}
 
 
 class SceneInterleaver(FrameInterleaver):
-    """FrameInterleaver.for_scene: `submit(ego_batch)`."""
+    """FrameInterleaver.for_scene: `submit(ego_batch)`, `submit(ego_batch, gt_boxes)` with evaluation."""
 
-    def submit(self, ego_batch):
-        return self._submit(ego_batch)
+    def submit(self, ego_batch, gt_boxes=None):
+        return self._submit(ego_batch, gt_boxes)
 
 
 class ScenePipeline(FramePipeline):
-    """FramePipeline.for_scene: `submit(ego_batch)`."""
+    """FramePipeline.for_scene: `submit(ego_batch)`, `submit(ego_batch, gt_boxes)` with evaluation."""
 
-    def submit(self, ego_batch):
-        return self._submit(ego_batch)
+    def submit(self, ego_batch, gt_boxes=None):
+        return self._submit(ego_batch, gt_boxes)
 
 
 class SceneGraphCache:
@@ -621,13 +740,15 @@ class SceneGraphCache:
     recently used first.  The key is the ordered `agent_modality_list` as a tuple (the ego first; the order is the fusion
     order).  `capture(slot, key)` makes slot `slot`'s graph for `key`."""
 
-    def __init__(self, sensor_type_dict, capacities, max_cav: int, voxel_limits, slots: int, max_graphs: int, capture):
+    def __init__(self, sensor_type_dict, capacities, max_cav: int, voxel_limits, slots: int, max_graphs: int, capture,
+                 gt_capacity=None):
         if int(max_graphs) < 1:
             raise ValueError(f"max_graphs {max_graphs}: a slot keeps at least one graph")
         self.sensors, self.capacities = dict(sensor_type_dict), dict(capacities)
         self.max_cav, self.voxel_limits, self.max_graphs = int(max_cav), voxel_limits, int(max_graphs)
         self.slots = [collections.OrderedDict() for _ in range(slots)]
         self.capture = capture
+        self.gt_capacity = gt_capacity                          # None: the graphs do not evaluate
         self.captures = 0
 
     def _spec(self, key):
@@ -642,11 +763,11 @@ class SceneGraphCache:
         self._spec(key)
         return key
 
-    def check(self, ego_batch):
+    def check(self, ego_batch, gt_boxes=None):
         """The key of a collated `batch_data['ego']`, after the checks of `key` and of `check_scene` for the frame's own list
-        (host only, nothing is copied)."""
+        and GT (host only, nothing is copied)."""
         key = tuple(ego_batch["agent_modality_list"])
-        check_scene(self._spec(key), key, self.voxel_limits, ego_batch)
+        check_scene(self._spec(key), key, self.voxel_limits, ego_batch, gt_boxes, self.gt_capacity)
         return key
 
     def graph(self, slot: int, key):
@@ -680,6 +801,13 @@ class SceneStream(FramePipeline):
             res = stream.submit(batch_data["ego"])      # None while the pipeline fills
         rest = stream.drain()
 
+    With `eval_thresholds` (and `gt_capacity`, see SceneGraph) every graph ends in the evaluation of its boxes:
+    `submit(ego_batch, gt_boxes)` takes the frame's GT from the reference's `post_processor.generate_gt_bbx(batch_data)`, and
+    `stream.result_stat` ({thr: {'tp', 'fp', 'score', 'gt'}}, the reference's format) gains each frame once, in frame order, when
+    `submit` / `drain` / `flush` hands it back.  A frame with no box adds its GT count only.  A frame with a union of area 0
+    raises ZeroDivisionError from that call, as the reference does, and is not appended.  The reference's
+    `eval_utils.eval_final_results(stream.result_stat, ...)` then gives the AP.
+
     `capacities` follows SceneGraph for every modality the stream may see; `pairwise_shape[1]` is max_cav.  Each slot keeps one
     captured SceneGraph per agent list, so a 2-agent frame runs a 2-agent graph and its result is bit for bit that of a
     SceneGraph captured for its list alone.  A list new to a slot is captured inside `submit` (a device synchronise and two eager
@@ -689,40 +817,46 @@ class SceneStream(FramePipeline):
     `check_scene` for its own list.
 
     Memory: the graphs of slot k are captured into one private pool, read slot k's one set of input buffers (every modality at
-    its capacity, for max_cav agents) and write slot k's one set of post-processing buffers, which lie outside the pool.  Graphs
+    its capacity, for max_cav agents) and write slot k's one set of post-processing (and evaluation) buffers, which lie outside
+    the pool.  Graphs
     of one slot never run at once (slot k's next frame waits for its last one's replay and copy-out), so they share their
     scratch.  A graph's static outputs may lie in another graph's scratch: a frame's device results are valid only until its
     slot's next replay.  The copy-out to the host happens before that; the host results are valid until the slot's next
     copy-out, `depth` submits later, as in FramePipeline."""
 
     def __init__(self, model, capacities, pairwise_shape, postprocess_params=None, depth: int = 2, max_graphs: int = 16,
-                 voxel_limits=None, device=None):
+                 voxel_limits=None, device=None, eval_thresholds=None, gt_capacity=None):
         from . import ops
         dev = device or next(model.parameters()).device
         depth = max(1, int(depth))
         self.model, self.capacities, self.pairwise_shape = model, dict(capacities), tuple(pairwise_shape)
         self.postprocess_params, self.voxel_limits = postprocess_params, voxel_limits
+        thresholds, self.gt_capacity = eval_setup(postprocess_params, eval_thresholds, gt_capacity)
         spec = scene_spec(model.sensor_type_dict, list(self.capacities), self.capacities)
         max_cav = int(self.pairwise_shape[1])
         self.cache = SceneGraphCache(model.sensor_type_dict, self.capacities, max_cav, _voxel_limits(model, spec, voxel_limits),
-                                     depth, max_graphs, self._capture)
+                                     depth, max_graphs, self._capture, self.gt_capacity)
         self.inputs = [_input_buffers({m: dict(sp, agents=max_cav) for m, sp in spec.items()}, dev) for _ in range(depth)]
         self.pools = [torch.cuda.graph_pool_handle() for _ in range(depth)]
         self.postprocess = [None] * depth
         if postprocess_params is not None:
             H, W, A = _anchor_box(postprocess_params).shape[:3]
             self.postprocess = [ops.PostprocessBuffers(H, W, A, 1000, dev) for _ in range(depth)]   # SceneGraph's `top`
+        self.evals = [None] * depth
+        if thresholds is not None:
+            self.evals = [FrameEval(1000, self.gt_capacity, dev) for _ in range(depth)]
         self.lists = [None] * depth                             # the agent list of the frame that last used each slot
-        self._start(self.cache.slots, [None] * depth, dev, 2)
+        self._start(self.cache.slots, [None] * depth, dev, 2, thresholds)
 
     def _capture(self, k, key):
         self.join(begin=False)          # the warm-up follows every frame in flight: slot k's last frame has left its buffers
         return SceneGraph(self.model, list(key), self.capacities, self.pairwise_shape, self.postprocess_params, device=self.dev,
                           voxel_limits=self.voxel_limits, inputs=self.inputs[k], pool=self.pools[k],
-                          postprocess_buffers=self.postprocess[k])
+                          postprocess_buffers=self.postprocess[k], eval_thresholds=self.eval_thresholds,
+                          gt_capacity=self.gt_capacity, eval_buffers=self.evals[k])
 
-    def _slot(self, k, ego_batch):
-        key = self.cache.check(ego_batch)
+    def _slot(self, k, ego_batch, gt_boxes=None):
+        key = self.cache.check(ego_batch, gt_boxes)
         g = self.cache.graph(k, key)
         self.lists[k] = key
         self._bind(k, g.results())
@@ -731,8 +865,8 @@ class SceneStream(FramePipeline):
     def _result(self, k):
         return {**self.host_out[k], "agent_modality_list": list(self.lists[k])}
 
-    def submit(self, ego_batch):
-        return self._submit(ego_batch)
+    def submit(self, ego_batch, gt_boxes=None):
+        return self._submit(ego_batch, gt_boxes)
 
     def capture(self, agent_modality_list):
         """Capture the graphs of an agent list in every slot ahead of the stream (a list a slot already holds is kept)."""

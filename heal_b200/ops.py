@@ -1746,9 +1746,10 @@ def box_decode_nms_late(cls_preds, reg_preds, dir_preds, anchors: torch.Tensor, 
 # detection evaluation (csrc/eval.cu): the TP / FP matching of eval_utils.caluclate_tp_fp for one frame
 # ------------------------------------------------------------------------------------------------
 class EvalBuffers:
-    """Caller-owned outputs + workspace of heal_eval_tp_fp, reusable for every frame of at most K detections and G GT boxes.
-    The outputs of a call share one byte buffer, `packed` = [status int32 | K sorted scores fp32 | (n_thr, K) TP flags uint8],
-    so one device-to-host copy brings all three back (`unpack`)."""
+    """Caller-owned outputs + workspace of heal_eval_tp_fp and heal_eval_tp_fp_counted, reusable for every frame of at most K
+    detections and G GT boxes (the capacities of eval_tp_fp_counted).  The outputs of a call share one byte buffer, `packed` =
+    [status int32 | K sorted scores fp32 | (n_thr, K) TP flags uint8] (K: the frame's count for eval_tp_fp, the detection
+    capacity for eval_tp_fp_counted), so one device-to-host copy brings all three back (`unpack`)."""
 
     def __init__(self, K: int, G: int, device):
         self.K, self.G = int(K), int(G)
@@ -1805,5 +1806,46 @@ def eval_tp_fp(det: torch.Tensor, scores: torch.Tensor, gt: torch.Tensor, thresh
     with _Prof("eval_tp_fp", 0, 24.0 * 4 * (K + G) + 4.0 * K * G * (1 + len(thr)) + (4.0 + len(thr)) * K):
         _call("heal_eval_tp_fp", _p(det), _p(scores), K, _p(gt), G, _host_f32(thr), len(thr), _p(buffers.out[4:]),
               _p(buffers.out[4 + 4 * K:]), _p(buffers.out), _p(buffers.workspace), buffers.workspace.numel())
+    buffers._bind(K, len(thr))
+    return buffers
+
+
+def _eval_count(t, name: str) -> torch.Tensor:
+    if not isinstance(t, torch.Tensor) or t.dtype != torch.int32 or tuple(t.shape) != (1,):
+        raise ValueError(f"eval_tp_fp_counted: {name} must be a (1,) int32 tensor")
+    _need_cuda(t)
+    return t
+
+
+@_guard
+def eval_tp_fp_counted(det: torch.Tensor, scores: torch.Tensor, count: torch.Tensor, gt: torch.Tensor, gt_count: torch.Tensor,
+                       thresholds: Sequence[float], buffers: Optional[EvalBuffers] = None) -> EvalBuffers:
+    """eval_tp_fp with the live sizes on the device, capture-safe (no host read): det (K_cap, 8, 3) and scores (K_cap,) of which
+    the first `count[0]` rows are live (e.g. PostprocessBuffers.boxes / .scores / .count), gt (G_cap, 8, 3) of which the first
+    `gt_count[0]` rows are live; count and gt_count (1,) int32 CUDA tensors.  Returns the buffers, bound at capacity: .packed =
+    [status | K_cap sorted scores | (n_thr, K_cap) flags], of which the first K scores and flags of each threshold are the frame's
+    (EvalBuffers.unpack(packed, K_cap, n_thr)).  A count above its capacity sets status bit HEAL_EVAL_OVER_CAPACITY = 2 and
+    writes no score or flag.  `buffers` (EvalBuffers(K, G) with K >= K_cap and G >= G_cap) are made when None; a captured graph
+    passes its own."""
+    _eval_boxes(det, "det")
+    _eval_boxes(gt, "gt")
+    K, G = det.shape[0], gt.shape[0]
+    if not isinstance(scores, torch.Tensor) or scores.dtype != torch.float32 or tuple(scores.shape) != (K,) \
+            or not scores.is_contiguous():
+        raise ValueError(f"eval_tp_fp_counted: scores must be a contiguous ({K},) fp32 tensor")
+    _need_cuda(scores)
+    _eval_count(count, "count")
+    _eval_count(gt_count, "gt_count")
+    if any(t.device != det.device for t in (scores, count, gt, gt_count)):
+        raise ValueError("eval_tp_fp_counted: det, scores, count, gt and gt_count must be on one device")
+    thr = [float(v) for v in thresholds]
+    if buffers is None:
+        buffers = EvalBuffers(K, G, det.device)
+    if buffers.K < K or buffers.G < G:
+        raise ValueError(f"eval_tp_fp_counted: buffers for K={buffers.K}, G={buffers.G}, the capacities are K={K}, G={G}")
+    with _Prof("eval_tp_fp", 0, 24.0 * 4 * (K + G) + 4.0 * K * G * (1 + len(thr)) + (4.0 + len(thr)) * K):
+        _call("heal_eval_tp_fp_counted", _p(det), _p(scores), _p(count), K, _p(gt), _p(gt_count), G, _host_f32(thr), len(thr),
+              _p(buffers.out[4:]), _p(buffers.out[4 + 4 * K:]), _p(buffers.out), _p(buffers.workspace),
+              buffers.workspace.numel())
     buffers._bind(K, len(thr))
     return buffers

@@ -491,6 +491,21 @@ int heal_eval_tp_fp(const float* det_corners, const float* det_scores, int K, co
                     const float* thresholds_host, int n_thr, float* sorted_scores_out, unsigned char* tp_out, int* status_out,
                     void* ws, size_t ws_bytes, void* stream);
 
+/* The same evaluation with the counts on the device, so that it can follow heal_box_decode_nms in one captured graph (no host
+ * read of the box count).  det_count, gt_count: device ints, the live K and G (e.g. the count_out of heal_box_decode_nms).
+ * K_cap, G_cap in [1, 4096]: host capacities.  det_corners (K_cap,8,3), det_scores (K_cap), gt_corners (G_cap,8,3): only the
+ * leading K / G rows are read.  Outputs at capacity: sorted_scores_out (K_cap), tp_out (n_thr, K_cap) (threshold t at
+ * tp_out + t * K_cap), leading K entries written, the rest left as they were.  Rules, tie order, NaN order and
+ * HEAL_EVAL_ZERO_UNION as heal_eval_tp_fp: for K <= K_cap and G <= G_cap the leading K scores and flags of every threshold equal
+ * heal_eval_tp_fp's on the leading rows bit for bit.  A count below 0 or above its capacity sets HEAL_EVAL_OVER_CAPACITY and
+ * writes no score and no flag (the counts are never clamped).  workspace >= heal_eval_workspace(K_cap, G_cap) bytes.  Launches
+ * four kernels whatever the counts; every argument is checked on the host (HEAL_ERR_ARG), nothing is read back. */
+#define HEAL_EVAL_OVER_CAPACITY 2
+int heal_eval_tp_fp_counted(const float* det_corners, const float* det_scores, const int* det_count, int K_cap,
+                            const float* gt_corners, const int* gt_count, int G_cap, const float* thresholds_host, int n_thr,
+                            float* sorted_scores_out, unsigned char* tp_out, int* status_out, void* ws, size_t ws_bytes,
+                            void* stream);
+
 /* ---- format conversion between fp32 and (split-)bf16 channels-last buffers -------------------
  * Any views: 4 channels at a time when channels, both channel strides and offsets (and split plane strides) are multiples of 4
  * and both data pointers are 16-byte aligned (fp32) or 8-byte aligned (bf16 / split), one channel at a time otherwise (same
