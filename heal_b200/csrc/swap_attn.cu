@@ -117,6 +117,11 @@ static inline bool aligned4(const heal_act_t* a) {
     return (a->cstride & 3) == 0 && (a->coffset & 3) == 0 && (a->fmt == 0 || (a->plane_stride & 3) == 0);
 }
 
+// the base pointer allows the 4-channel vector accesses of act_load4 / act_store4 (16 bytes fp32, 8 bytes bf16)
+static inline bool data_aligned4(const heal_act_t* a) {
+    return ((uintptr_t)a->data % (a->fmt == 0 ? 16u : 8u)) == 0;
+}
+
 }  // namespace
 
 extern "C" int heal_swap_attention(const heal_act_t* qkv, const int* n_agents_host, int B, int L, int H, int W, int C,
@@ -124,8 +129,11 @@ extern "C" int heal_swap_attention(const heal_act_t* qkv, const int* n_agents_ho
     if (!qkv || !qkv->data || !n_agents_host || !bias || !out || !out->data) return HEAL_ERR_ARG;
     if (B < 0 || L < 1 || H < 1 || W < 1 || C < 1 || window_size < 1 || (H % window_size) || (W % window_size)) return HEAL_ERR_ARG;
     if ((C % DH) || L * window_size * window_size > MAX_TOK || !aligned4(qkv) || !aligned4(out)) return HEAL_ERR_UNSUPPORTED;
+    if (!data_aligned4(qkv) || !data_aligned4(out)) return HEAL_ERR_UNSUPPORTED;
     const long long windows = (long long)(H / window_size) * (W / window_size);
     if (C / DH > 65535 || windows > 0x7fffffffLL) return HEAL_ERR_UNSUPPORTED;
+    for (int b = 0; b < B; ++b)          // every count before the first launch, so a bad one leaves the output untouched
+        if (n_agents_host[b] < 1 || n_agents_host[b] > L) return HEAL_ERR_ARG;
     SwapP p;
     p.qkv = to_view(qkv); p.out = to_view(out); p.bias = bias;
     p.H = H; p.W = W; p.C = C; p.L = L; p.w = window_size; p.grid = grid_mode ? 1 : 0;
@@ -135,10 +143,7 @@ extern "C" int heal_swap_attention(const heal_act_t* qkv, const int* n_agents_ho
     for (int b0 = 0; b0 < B; b0 += SCENES) {
         const int nb = B - b0 < SCENES ? B - b0 : SCENES;
         p.b0 = b0;
-        for (int z = 0; z < nb; ++z) {
-            if (n_agents_host[b0 + z] < 1 || n_agents_host[b0 + z] > L) return HEAL_ERR_ARG;
-            p.nb[z] = n_agents_host[b0 + z];
-        }
+        for (int z = 0; z < nb; ++z) p.nb[z] = n_agents_host[b0 + z];
         k_swap_attention<<<dim3((unsigned)windows, (unsigned)(C / DH), (unsigned)nb), threads, 0, (cudaStream_t)stream_>>>(p);
         ++launches;
     }

@@ -415,9 +415,10 @@ __global__ void __launch_bounds__(256) k_split_combine(CombP p) {
 // ---- STTF resample ---------------------------------------------------------------------------------------------------
 struct SttfP { ActV src, out; const float* theta; int H, W, C; };
 
-// torch.linspace(-1, 1, n) in fp32 (the base grid of F.affine_grid with align_corners=True)
+// torch.linspace(-1, 1, n) in fp32 (the base grid of F.affine_grid with align_corners=True); F.affine_grid uses 0 for an axis of
+// one pixel, not linspace's -1
 __device__ __forceinline__ float linspace_pm1(int i, int n) {
-    if (n == 1) return -1.f;
+    if (n == 1) return 0.f;
     const float step = 2.f / (float)(n - 1);
     return i < n / 2 ? -1.f + step * (float)i : 1.f - step * (float)(n - 1 - i);
 }
@@ -516,6 +517,7 @@ extern "C" int heal_split_attn(const heal_act_t* o, const heal_act_t* x, int n_i
     if (!o || !o->data || !x || !x->data || !out || !out->data || !fc1_t || !ln_w || !ln_b || !fc2_t || !workspace) return HEAL_ERR_ARG;
     if (n_img < 0 || H < 1 || W < 1 || !fmt_ok(o) || !fmt_ok(x) || !fmt_ok(out)) return HEAL_ERR_ARG;
     if (C != SPLIT_C || !aligned_to(o, 4) || !aligned_to(x, 4) || !aligned_to(out, 4)) return HEAL_ERR_UNSUPPORTED;
+    if (n_img > 65535) return HEAL_ERR_UNSUPPORTED;      // gridDim.y of the pool and combine launches
     if (!data_aligned(o, 4) || !data_aligned(x, 4) || !data_aligned(out, 4) || ((uintptr_t)workspace & 15)) return HEAL_ERR_UNSUPPORTED;
     if (ws_bytes < heal_split_attn_workspace(n_img, C)) return HEAL_ERR_WORKSPACE;
     if (n_img == 0) return HEAL_OK;
