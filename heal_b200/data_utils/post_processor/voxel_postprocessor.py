@@ -13,6 +13,18 @@ import torch
 
 from ... import ops
 
+TOP = 1000          # decode capacity: the best-scoring candidates kept for NMS (box_utils.nms_rotated's `top`)
+
+
+def decode_kwargs(params, has_dir: bool):
+    """The keyword arguments ops.box_decode_nms, box_decode_nms_multi and box_decode_nms_late take from a `postprocess:` block:
+    thresholds, box order, range mask, capacity TOP, and the direction-bin correction of `dir_args` when the heads have a dir
+    head."""
+    dargs = params.get('dir_args', {}) if has_dir else {}
+    return dict(score_threshold=params['target_args']['score_threshold'], nms_threshold=params['nms_thresh'],
+                dir_offset=dargs.get('dir_offset', 0.0), num_bins=dargs.get('num_bins', 2), order=params['order'],
+                gt_range=params['gt_range'], top=TOP)
+
 
 class VoxelPostprocessor:
     def __init__(self, anchor_params, train):
@@ -68,11 +80,8 @@ class VoxelPostprocessor:
         A, H, W = cavs[0]["cls"].shape[1], cavs[0]["cls"].shape[2], cavs[0]["cls"].shape[3]
         bkey = (H * len(cavs), W, A, str(cavs[0]["cls"].device))
         if bkey not in self._buffers:
-            self._buffers[bkey] = ops.PostprocessBuffers(H * len(cavs), W, A, 1000, cavs[0]["cls"].device)
-        dargs = self.params.get('dir_args', {}) if any(dirs) else {}
-        return ops.box_decode_nms_multi(cavs, self.params['target_args']['score_threshold'], self.params['nms_thresh'],
-                                        dir_offset=dargs.get('dir_offset', 0.0), num_bins=dargs.get('num_bins', 2),
-                                        order=self.params['order'], gt_range=self.params['gt_range'], top=1000, buffers=self._buffers[bkey])
+            self._buffers[bkey] = ops.PostprocessBuffers(H * len(cavs), W, A, TOP, cavs[0]["cls"].device)
+        return ops.box_decode_nms_multi(cavs, **decode_kwargs(self.params, any(dirs)), buffers=self._buffers[bkey])
 
     def _decode_one(self, cav_content, out):
         cls = out.get('cls_preds', out.get('psm'))
@@ -87,12 +96,9 @@ class VoxelPostprocessor:
         A, H, W = cls.shape[1], cls.shape[2], cls.shape[3]
         bkey = (H, W, A, str(dev))
         if bkey not in self._buffers:
-            self._buffers[bkey] = ops.PostprocessBuffers(H, W, A, 1000, dev)
-        dargs = self.params.get('dir_args', {}) if dirp is not None else {}
+            self._buffers[bkey] = ops.PostprocessBuffers(H, W, A, TOP, dev)
         return ops.box_decode_nms(cls, reg, dirp, anchors, cav_content['transformation_matrix'],
-                                  self.params['target_args']['score_threshold'], self.params['nms_thresh'],
-                                  dir_offset=dargs.get('dir_offset', 0.0), num_bins=dargs.get('num_bins', 2),
-                                  order=self.params['order'], gt_range=self.params['gt_range'], top=1000, buffers=self._buffers[bkey])
+                                  **decode_kwargs(self.params, dirp is not None), buffers=self._buffers[bkey])
 
     def _device_anchors(self, anchor, dev):
         """fp32 device copy of the anchor grid, cached per (shape, device).  The reference's collate builds a NEW anchor tensor for

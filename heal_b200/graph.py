@@ -12,32 +12,73 @@ import numbers
 
 import torch
 
+from . import ops
 from ._lib import lib
+from .data_utils.post_processor.voxel_postprocessor import TOP, VoxelPostprocessor, decode_kwargs
+
+
+def warm_up(run, device):
+    """Two eager calls of `run` on a side stream under no_grad, then a device synchronise: the first launches load modules and
+    build lazy caches outside any capture, and outside a capture's private memory pool."""
+    side = torch.cuda.Stream(device=device)
+    side.wait_stream(torch.cuda.current_stream(device))
+    with torch.cuda.stream(side), torch.no_grad():
+        for _ in range(2):
+            run()
+    torch.cuda.current_stream(device).wait_stream(side)
+    torch.cuda.synchronize(device)
+
+
+def record(run, pool=None):
+    """Capture one call of `run` into a CUDA graph, in the private memory pool `pool` (torch.cuda.graph_pool_handle()) when
+    given.  Returns (graph, the output of `run`, kernels launched per replay)."""
+    graph = torch.cuda.CUDAGraph()
+    l0 = lib.heal_launch_count()
+    with torch.no_grad(), torch.cuda.graph(graph, pool=pool, capture_error_mode="thread_local"):
+        out = run()
+    return graph, out, int(lib.heal_launch_count() - l0)
+
+
+def capture(run, device, pool=None):
+    """`warm_up` then `record`: (graph, output, kernels per replay) of `run`."""
+    warm_up(run, device)
+    return record(run, pool)
+
+
+def _heads(out):
+    """The heads of a model's output dict, by name."""
+    return {k: out[k] for k in ("cls_preds", "reg_preds", "dir_preds") if k in out}
+
+
+def _anchors(postprocess_params, device):
+    """VoxelPostprocessor's anchor grid (H, W, A, 7) for `postprocess_params`, fp32 on `device`."""
+    grid = VoxelPostprocessor(postprocess_params, False).generate_anchor_box()
+    return torch.from_numpy(grid).to(device=device, dtype=torch.float32).contiguous()
+
+
+def _join(device, streams, begin: bool):
+    """Order `streams` after (begin) / before (end) the current stream of `device`, e.g. around timing events."""
+    cur = torch.cuda.current_stream(device)
+    for s in streams:
+        if begin:
+            s.wait_stream(cur)
+        else:
+            cur.wait_stream(s)
 
 
 class GraphedCall:
     """Generic capture: `fn(build(buffers))` over named static input buffers.  `spec` maps a name to (shape, dtype);
     names in `varlen` may be loaded with fewer rows than their capacity (prefix copy; the live length travels in another input,
-    e.g. `agent_offsets[-1]`).  Used by bench.py for the single-agent / SECOND / camera workloads."""
+    e.g. `agent_offsets[-1]`); `init` is loaded before the capture.  Used by bench.py for the single-agent / SECOND / camera
+    workloads."""
 
-    def __init__(self, fn, spec, build, device, varlen=(), init=None, warmup=2):
+    def __init__(self, fn, spec, build, device, varlen=(), init=None):
         self.bufs = {k: torch.zeros(tuple(shape), dtype=dt, device=device) for k, (shape, dt) in spec.items()}
         self.varlen = set(varlen)
         if init is not None:
-            self.load(**init)
+            GraphedCall.load(self, **init)          # by name, whatever a subclass's `load` takes
         self.data = build(self.bufs)
-        side = torch.cuda.Stream(device=device)
-        side.wait_stream(torch.cuda.current_stream(device))
-        with torch.cuda.stream(side), torch.no_grad():
-            for _ in range(warmup):
-                fn(self.data)
-        torch.cuda.current_stream(device).wait_stream(side)
-        torch.cuda.synchronize(device)
-        self.graph = torch.cuda.CUDAGraph()
-        l0 = lib.heal_launch_count()
-        with torch.no_grad(), torch.cuda.graph(self.graph, capture_error_mode="thread_local"):
-            self.out = fn(self.data)
-        self.kernels_per_replay = int(lib.heal_launch_count() - l0)
+        self.graph, self.out, self.kernels_per_replay = capture(lambda: fn(self.data), device)
 
     def load(self, **tensors):
         nbytes = 0
@@ -57,45 +98,32 @@ class GraphedCall:
         return self.out
 
 
-class FrameGraph:
-    def __init__(self, model, n_agents: int, point_capacity: int, pairwise_shape, modality: str = "m1", forward_fn=None,
-                 device=None, warmup: int = 2):
+class FrameGraph(GraphedCall):
+    """One frame of `n_agents` agents of one lidar modality: `model` over the static inputs `points` (up to `point_capacity`
+    rows; the live count travels in `agent_offsets[-1]`), `agent_offsets` and `pairwise` (identities until the first load)."""
+
+    def __init__(self, model, n_agents: int, point_capacity: int, pairwise_shape, modality: str = "m1", device=None):
         dev = device or next(model.parameters()).device
-        self.points = torch.zeros((point_capacity, 4), dtype=torch.float32, device=dev)
-        self.offsets = torch.zeros((n_agents + 1,), dtype=torch.int32, device=dev)
-        self.pairwise = torch.zeros(tuple(pairwise_shape), dtype=torch.float64, device=dev)
+        spec = {"points": ((point_capacity, 4), torch.float32), "agent_offsets": ((n_agents + 1,), torch.int32),
+                "pairwise": (tuple(pairwise_shape), torch.float64)}
+
+        def build(b):
+            return {f"inputs_{modality}": {"points": b["points"], "agent_offsets": b["agent_offsets"]},
+                    "agent_modality_list": [modality] * n_agents, "record_len": [n_agents], "pairwise_t_matrix": b["pairwise"]}
         self.capacity = point_capacity
-        self.data = {f"inputs_{modality}": {"points": self.points, "agent_offsets": self.offsets},
-                     "agent_modality_list": [modality] * n_agents, "record_len": [n_agents],
-                     "pairwise_t_matrix": self.pairwise}
-        fn = forward_fn or model
-        self.pairwise.copy_(torch.eye(4, dtype=torch.float64, device=dev).expand(self.pairwise.shape))
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side), torch.no_grad():
-            for _ in range(warmup):
-                fn(self.data)
-        torch.cuda.current_stream(dev).wait_stream(side)
-        torch.cuda.synchronize(dev)
-        self.graph = torch.cuda.CUDAGraph()
-        l0 = lib.heal_launch_count()
-        with torch.no_grad(), torch.cuda.graph(self.graph, capture_error_mode="thread_local"):
-            self.out = fn(self.data)
-        self.kernels_per_replay = int(lib.heal_launch_count() - l0)
+        super().__init__(model, spec, build, dev, varlen=("points",),
+                         init={"pairwise": torch.eye(4, dtype=torch.float64, device=dev).expand(tuple(pairwise_shape))})
 
     def load(self, points: torch.Tensor, offsets: torch.Tensor, pairwise: torch.Tensor):
-        """points (P,4) f32, offsets (A+1) i32, pairwise f64 — device or pinned-host tensors (async copies on the current stream)."""
-        n = points.shape[0]
-        if n > self.capacity:
-            raise ValueError(f"scene has {n} points, graph capacity is {self.capacity}")
-        self.points[:n].copy_(points, non_blocking=True)
-        self.offsets.copy_(offsets, non_blocking=True)
-        self.pairwise.copy_(pairwise, non_blocking=True)
-        return sum(t.numel() * t.element_size() for t in (points, offsets, pairwise))
+        """points (P,4) f32, offsets (A+1) i32, pairwise f64 — device or pinned-host tensors (async copies on the current stream).
+        Returns the bytes copied."""
+        if points.shape[0] > self.capacity:
+            raise ValueError(f"scene has {points.shape[0]} points, graph capacity is {self.capacity}")
+        return super().load(points=points, agent_offsets=offsets, pairwise=pairwise)
 
-    def replay(self):
-        self.graph.replay()
-        return self.out
+    def results(self):
+        """The device tensors a frame's consumer reads: the heads."""
+        return _heads(self.out)
 
 
 class FrameInterleaver:
@@ -111,16 +139,11 @@ class FrameInterleaver:
         dev = device or next(model.parameters()).device
         self._start([FrameGraph(model, n_agents, point_capacity, pairwise_shape, modality, device=dev) for _ in range(n)], dev)
 
-    @classmethod
-    def for_scene(cls, model, agent_modality_list, capacities, pairwise_shape, postprocess_params=None, n: int = 2,
-                  device=None, **graph_kwargs):
-        """N captured SceneGraphs of a mixed-modality scene; `submit(ego_batch)` (`submit(ego_batch, gt_boxes)` with
-        `eval_thresholds`) loads and replays one."""
-        dev = device or next(model.parameters()).device
-        il = SceneInterleaver.__new__(SceneInterleaver)
-        il._start([SceneGraph(model, agent_modality_list, capacities, pairwise_shape, postprocess_params, device=dev,
-                              **graph_kwargs) for _ in range(n)], dev)
-        return il
+    @staticmethod
+    def for_scene(*args, **kwargs):
+        """N captured SceneGraphs of a mixed-modality scene: SceneInterleaver(model, agent_modality_list, capacities,
+        pairwise_shape, postprocess_params=None, n=2, device=None, **graph_kwargs)."""
+        return SceneInterleaver(*args, **kwargs)
 
     def _start(self, graphs, dev):
         self.dev, self.n = dev, len(graphs)
@@ -145,12 +168,8 @@ class FrameInterleaver:
         return out
 
     def join(self, begin: bool):
-        cur = torch.cuda.current_stream(self.dev)
-        for s in self.streams:
-            if begin:
-                s.wait_stream(cur)
-            else:
-                cur.wait_stream(s)
+        """Order the interleaver's streams after (begin) / before (end) the caller's current stream."""
+        _join(self.dev, self.streams, begin)
 
 
 class FramePipeline:
@@ -167,37 +186,25 @@ class FramePipeline:
     Each frame's result is complete on the host before its buffers are reused (events, no host sync inside submit).
     """
 
-    OUT_KEYS = ("cls_preds", "reg_preds", "dir_preds")
-
     def __init__(self, model, n_agents: int, point_capacity: int, pairwise_shape, modality: str = "m1", device=None,
                  compute_streams: int = 2, depth: int = 2):
         """`depth` = captured frames (slots) in flight: `submit` of frame i returns the predictions of frame i - (depth - 1).
         depth 2 keeps one frame queued behind the running one; deeper pipelines keep both compute streams fed while the host
         waits for a result (on C2 depths 2-4 measure the same within run-to-run noise, 290-305 frames/s end to end)."""
         dev = device or next(model.parameters()).device
-        graphs = [FrameGraph(model, n_agents, point_capacity, pairwise_shape, modality, device=dev) for _ in range(max(2, int(depth)))]
-        self._start(graphs, [{k: g.out[k] for k in self.OUT_KEYS if k in g.out} for g in graphs], dev, compute_streams)
+        self._start([FrameGraph(model, n_agents, point_capacity, pairwise_shape, modality, device=dev)
+                     for _ in range(max(2, int(depth)))], dev, compute_streams)
 
-    @classmethod
-    def for_scene(cls, model, agent_modality_list, capacities, pairwise_shape, postprocess_params=None, device=None,
-                  compute_streams: int = 2, depth: int = 2, eval_thresholds=None, gt_capacity=None, **graph_kwargs):
-        """The pipeline over a mixed-modality scene (SceneGraph slots): `submit(ego_batch)` takes the reference's collated
-        `batch_data['ego']` and returns, pinned on the host, the boxes, scores and box count of frame i - (depth - 1) when
-        `postprocess_params` is given (`boxes[:count[0]]`), else its heads.  With `eval_thresholds` (and `gt_capacity`, see
-        SceneGraph) `submit(ego_batch, gt_boxes)` also takes the frame's GT, each frame is evaluated in its graph, and
-        `pipe.result_stat` collects the frames in the reference's format as they come back."""
-        dev = device or next(model.parameters()).device
-        graphs = [SceneGraph(model, agent_modality_list, capacities, pairwise_shape, postprocess_params, device=dev,
-                             eval_thresholds=eval_thresholds, gt_capacity=gt_capacity, **graph_kwargs)
-                  for _ in range(max(2, int(depth)))]
-        pipe = ScenePipeline.__new__(ScenePipeline)
-        pipe._start(graphs, [g.results() for g in graphs], dev, compute_streams, graphs[0].eval_thresholds)
-        return pipe
+    @staticmethod
+    def for_scene(*args, **kwargs):
+        """The pipeline over a mixed-modality scene: ScenePipeline(model, agent_modality_list, capacities, pairwise_shape,
+        postprocess_params=None, device=None, compute_streams=2, depth=2, **graph_kwargs), e.g. `eval_thresholds`."""
+        return ScenePipeline(*args, **kwargs)
 
-    def _start(self, graphs, results, dev, compute_streams, eval_thresholds=None):
-        """`results[k]`: the device tensors slot k copies back to the host after each replay, by name (None: bound later by
-        `_bind`, when the slot's first graph exists).  With `eval_thresholds` the results carry each frame's evaluation
-        (SceneGraph.results), which goes into `result_stat` as the frame is handed back."""
+    def _start(self, graphs, dev, compute_streams, eval_thresholds=None):
+        """Slot k replays `graphs[k]` and copies its `results()` (device tensors by name) back to the host after each replay; a
+        None slot is bound by `_bind` when a frame gives it a graph.  With `eval_thresholds` the results carry each frame's
+        evaluation (SceneGraph.results), which goes into `result_stat` as the frame is handed back."""
         self.dev, self.depth = dev, len(graphs)
         self.eval_thresholds = eval_thresholds
         self.result_stat = None if eval_thresholds is None else \
@@ -214,12 +221,10 @@ class FramePipeline:
         self.count = 0
         self.h2d_bytes = 0
         self.d2h_bytes = 0
-        for k, r in enumerate(results):
-            if r is not None:
-                self._bind(k, r)
-        cur = torch.cuda.current_stream(dev)
-        for s in (self.s_in, *set(self.s_comp), self.s_out):
-            s.wait_stream(cur)
+        for k, g in enumerate(graphs):
+            if g is not None:
+                self._bind(k, g.results())
+        self.join(begin=True)
 
     def _bind(self, k, results):
         """Slot k copies `results` (device tensors by name) into its pinned host tensors after each replay."""
@@ -295,12 +300,7 @@ class FramePipeline:
 
     def join(self, begin: bool):
         """Order the pipeline's streams after (begin) / before (end) the caller's current stream, e.g. around timing events."""
-        cur = torch.cuda.current_stream(self.dev)
-        for s in (self.s_in, *set(self.s_comp), self.s_out):
-            if begin:
-                s.wait_stream(cur)
-            else:
-                cur.wait_stream(s)
+        _join(self.dev, (self.s_in, *self.s_comp, self.s_out), begin)
 
 
 def _count(v):
@@ -383,12 +383,6 @@ def _voxel_limits(model, spec, voxel_limits):
     return out
 
 
-def _anchor_box(postprocess_params):
-    """The anchors (H, W, A, 7) of VoxelPostprocessor for `postprocess_params`, on the host."""
-    from .data_utils.post_processor.voxel_postprocessor import VoxelPostprocessor
-    return VoxelPostprocessor(postprocess_params, False).generate_anchor_box()
-
-
 def eval_setup(postprocess_params, eval_thresholds, gt_capacity):
     """(thresholds, GT capacity) of a captured frame that evaluates its boxes, or (None, None) when `eval_thresholds` is None.
     Checked on the host: evaluation needs `postprocess_params`; 1 to 8 thresholds, each > 0; the GT capacity is `gt_capacity`,
@@ -432,18 +426,16 @@ def check_gt(gt_boxes, gt_capacity):
 
 class FrameEval:
     """The evaluation of a captured frame: its static GT input (`gt` (capacity, 8, 3) fp32 corners, `gt_count` (1,) int32) and
-    the ops.EvalBuffers heal_eval_tp_fp_counted writes, for up to `det_capacity` boxes (the post-processing's `top`).  Caller-owned
+    the ops.EvalBuffers heal_eval_tp_fp_counted writes, for up to `det_capacity` boxes (the decode capacity TOP).  Caller-owned
     so that several graphs can share one (SceneStream: one per pipeline slot, outside the graph pool)."""
 
     def __init__(self, det_capacity: int, gt_capacity: int, device):
-        from . import ops
         self.gt = torch.zeros((gt_capacity, 8, 3), dtype=torch.float32, device=device)
         self.gt_count = torch.zeros((1,), dtype=torch.int32, device=device)
         self.buffers = ops.EvalBuffers(det_capacity, gt_capacity, device)
 
     def run(self, post, thresholds):
         """Match the post-processed boxes (ops.PostprocessBuffers: boxes, scores, count on the device) to the GT; capture-safe."""
-        from . import ops
         return ops.eval_tp_fp_counted(post.boxes, post.scores, post.count, self.gt, self.gt_count, thresholds, self.buffers)
 
     def load(self, gt_boxes):
@@ -465,9 +457,9 @@ class LateFusionGraph:
 
     With `eval_thresholds` (e.g. inference.py's (0.3, 0.5, 0.7)) the graph ends in heal_eval_tp_fp_counted, which matches the
     boxes to the GT given to `load(batch_data, gt_boxes)`: `g.eval.buffers.packed` holds the frame's status, sorted scores and
-    flags at the capacity `top` (eval_utils.append_packed turns a host copy into `result_stat` entries).  Late fusion's GT is the
-    union of every cav's objects, so `gt_capacity` (default `postprocess_params['max_num']`) may need to be larger than an
-    intermediate-fusion frame's.
+    flags at the decode capacity TOP (eval_utils.append_packed turns a host copy into `result_stat` entries).  Late fusion's GT
+    is the union of every cav's objects, so `gt_capacity` (default `postprocess_params['max_num']`) may need to be larger than
+    an intermediate-fusion frame's.
     `capacities[m]`: for a lidar modality the point capacity of ALL its cavs together (raw clouds, `points` + `agent_offsets`; the
     live counts travel in the offsets), for a camera modality (cameras, image height, image width) per cav for normalised fp32
     images, or (cameras, frame height, frame width, torch.uint8) for raw uint8 (H0, W0, 3) frames, which the encoder resizes, crops
@@ -475,13 +467,11 @@ class LateFusionGraph:
 
     CAMERA_KEYS = ("rots", "trans", "intrins", "post_rots", "post_trans")
 
-    def __init__(self, model, modality_of_each_cav, capacities, postprocess_params, device=None, warmup: int = 2, top: int = 1000,
-                 eval_thresholds=None, gt_capacity=None):
-        from . import ops
-        from .data_utils.post_processor.voxel_postprocessor import VoxelPostprocessor
+    def __init__(self, model, modality_of_each_cav, capacities, postprocess_params, device=None, eval_thresholds=None,
+                 gt_capacity=None):
         dev = device or next(model.parameters()).device
         self.eval_thresholds, self.gt_capacity = eval_setup(postprocess_params, eval_thresholds, gt_capacity)
-        self.eval = FrameEval(top, self.gt_capacity, dev) if self.eval_thresholds is not None else None
+        self.eval = FrameEval(TOP, self.gt_capacity, dev) if self.eval_thresholds is not None else None
         self.modalities = list(modality_of_each_cav)
         n = len(self.modalities)
         self.groups = {}
@@ -489,36 +479,20 @@ class LateFusionGraph:
             self.groups.setdefault(m, []).append(i)
         self.inputs = _input_buffers(scene_spec(model.sensor_type_dict, self.modalities, capacities), dev)
         self.transforms = torch.eye(4, dtype=torch.float32, device=dev).repeat(n, 1, 1).contiguous()
-        pp = VoxelPostprocessor(postprocess_params, False)
-        self.anchors = torch.from_numpy(pp.generate_anchor_box()).to(device=dev, dtype=torch.float32).contiguous()
+        self.anchors = _anchors(postprocess_params, dev)
         A = self.anchors.shape[2]
-        dargs = postprocess_params.get('dir_args', {})
-        bins = int(dargs.get('num_bins', 2))
-        self.buffers = ops.PostprocessBuffers(self.anchors.shape[0] * n, self.anchors.shape[1], A, top, dev)
+        self.buffers = ops.PostprocessBuffers(self.anchors.shape[0] * n, self.anchors.shape[1], A, TOP, dev)
+        decode = decode_kwargs(postprocess_params, True)       # the grouped heads always carry the dir channels
 
         def run():
             y, _ = model.grouped_heads(self.groups, self.inputs, n)
-            post = ops.box_decode_nms_late(y, y, y, self.anchors, self.transforms,
-                                           postprocess_params['target_args']['score_threshold'], postprocess_params['nms_thresh'],
-                                           dir_offset=dargs.get('dir_offset', 0.0), num_bins=bins, order=postprocess_params['order'],
-                                           gt_range=postprocess_params['gt_range'], top=top, buffers=self.buffers,
+            post = ops.box_decode_nms_late(y, y, y, self.anchors, self.transforms, **decode, buffers=self.buffers,
                                            coffsets=(0, A, 8 * A))
             if self.eval is not None:
                 self.eval.run(post, self.eval_thresholds)
             return post
 
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side), torch.no_grad():
-            for _ in range(warmup):
-                run()
-        torch.cuda.current_stream(dev).wait_stream(side)
-        torch.cuda.synchronize(dev)
-        self.graph = torch.cuda.CUDAGraph()
-        l0 = lib.heal_launch_count()
-        with torch.no_grad(), torch.cuda.graph(self.graph, capture_error_mode="thread_local"):
-            self.out = run()
-        self.kernels_per_replay = int(lib.heal_launch_count() - l0)
+        self.graph, self.out, self.kernels_per_replay = capture(run, dev)
 
     def load(self, batch_data, gt_boxes=None):
         """Copy a scene's inputs and cav -> ego transforms into the captured buffers (asynchronous copies on the current stream).
@@ -631,12 +605,12 @@ class SceneGraph:
     GT comes in with `load(ego_batch, gt_boxes)`: (G, 8, 3) fp32 corners, what the reference's
     `post_processor.generate_gt_bbx(batch_data)` returns on the host, copied into a static (gt_capacity, 8, 3) buffer and a
     device count.  `gt_capacity` defaults to `postprocess_params['max_num']` and must be given when that key is absent.
-    `results()` then adds the packed evaluation (ops.EvalBuffers: status, sorted scores, flags at capacity `top`) and G."""
+    `results()` then adds the packed evaluation (ops.EvalBuffers: status, sorted scores, flags at the decode capacity TOP)
+    and G."""
 
     def __init__(self, model, agent_modality_list, capacities, pairwise_shape, postprocess_params=None, device=None,
-                 voxel_limits=None, warmup: int = 2, top: int = 1000, inputs=None, pool=None, postprocess_buffers=None,
-                 eval_thresholds=None, gt_capacity=None, eval_buffers=None):
-        from . import ops
+                 voxel_limits=None, inputs=None, pool=None, postprocess_buffers=None, eval_thresholds=None, gt_capacity=None,
+                 eval_buffers=None):
         dev = device or next(model.parameters()).device
         self.eval_thresholds, self.gt_capacity = eval_setup(postprocess_params, eval_thresholds, gt_capacity)
         self.modalities = list(agent_modality_list)
@@ -651,39 +625,25 @@ class SceneGraph:
                      "record_len": [n], "pairwise_t_matrix": self.pairwise}
         self.postprocess = None
         if postprocess_params is not None:
-            self.anchors = torch.from_numpy(_anchor_box(postprocess_params)).to(device=dev, dtype=torch.float32).contiguous()
+            self.anchors = _anchors(postprocess_params, dev)
             H, W, A = self.anchors.shape[:3]
-            self.postprocess = ops.PostprocessBuffers(H, W, A, top, dev) if postprocess_buffers is None else postprocess_buffers
+            self.postprocess = ops.PostprocessBuffers(H, W, A, TOP, dev) if postprocess_buffers is None else postprocess_buffers
         self.eval = None
         if self.eval_thresholds is not None:
-            self.eval = FrameEval(top, self.gt_capacity, dev) if eval_buffers is None else eval_buffers
+            self.eval = FrameEval(TOP, self.gt_capacity, dev) if eval_buffers is None else eval_buffers
         pparams, eye = postprocess_params, torch.eye(4, dtype=torch.float64)
 
         def run():
             out = model(self.data)
             if pparams is not None:                     # VoxelPostprocessor._decode_one for the ego
-                dargs = pparams.get('dir_args', {}) if out.get('dir_preds') is not None else {}
-                out['postprocess'] = ops.box_decode_nms(
-                    out['cls_preds'], out['reg_preds'], out.get('dir_preds'), self.anchors, eye,
-                    pparams['target_args']['score_threshold'], pparams['nms_thresh'], dir_offset=dargs.get('dir_offset', 0.0),
-                    num_bins=dargs.get('num_bins', 2), order=pparams['order'], gt_range=pparams['gt_range'], top=top,
-                    buffers=self.postprocess)
+                dirp = out.get('dir_preds')
+                out['postprocess'] = ops.box_decode_nms(out['cls_preds'], out['reg_preds'], dirp, self.anchors, eye,
+                                                        **decode_kwargs(pparams, dirp is not None), buffers=self.postprocess)
                 if self.eval is not None:
                     self.eval.run(out['postprocess'], self.eval_thresholds)
             return out
 
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side), torch.no_grad():
-            for _ in range(warmup):
-                run()
-        torch.cuda.current_stream(dev).wait_stream(side)
-        torch.cuda.synchronize(dev)
-        self.graph = torch.cuda.CUDAGraph()
-        l0 = lib.heal_launch_count()
-        with torch.no_grad(), torch.cuda.graph(self.graph, pool=pool, capture_error_mode="thread_local"):
-            self.out = run()
-        self.kernels_per_replay = int(lib.heal_launch_count() - l0)
+        self.graph, self.out, self.kernels_per_replay = capture(run, dev, pool)
 
     def load(self, ego_batch, gt_boxes=None):
         """Copy a scene's inputs and pairwise transforms (and with evaluation its GT corners) into the captured buffers
@@ -712,24 +672,42 @@ class SceneGraph:
 
     def results(self):
         """The device tensors a frame's consumer reads: the ego's boxes, scores and box count with `postprocess_params`, else
-        the heads; with evaluation also `eval` (EvalBuffers.packed at capacity `top`) and `gt_count`."""
+        the heads; with evaluation also `eval` (EvalBuffers.packed at capacity TOP) and `gt_count`."""
         if self.postprocess is not None:
             out = {"boxes": self.postprocess.boxes, "scores": self.postprocess.scores, "count": self.postprocess.count}
             if self.eval is not None:
                 out.update(eval=self.eval.buffers.packed, gt_count=self.eval.gt_count)
             return out
-        return {k: self.out[k] for k in FramePipeline.OUT_KEYS if k in self.out}
+        return _heads(self.out)
 
 
 class SceneInterleaver(FrameInterleaver):
-    """FrameInterleaver.for_scene: `submit(ego_batch)`, `submit(ego_batch, gt_boxes)` with evaluation."""
+    """N captured SceneGraphs of a mixed-modality scene on N streams (FrameInterleaver.for_scene): `submit(ego_batch)`
+    (`submit(ego_batch, gt_boxes)` with `eval_thresholds`) loads and replays one."""
+
+    def __init__(self, model, agent_modality_list, capacities, pairwise_shape, postprocess_params=None, n: int = 2,
+                 device=None, **graph_kwargs):
+        dev = device or next(model.parameters()).device
+        self._start([SceneGraph(model, agent_modality_list, capacities, pairwise_shape, postprocess_params, device=dev,
+                                **graph_kwargs) for _ in range(n)], dev)
 
     def submit(self, ego_batch, gt_boxes=None):
         return self._submit(ego_batch, gt_boxes)
 
 
 class ScenePipeline(FramePipeline):
-    """FramePipeline.for_scene: `submit(ego_batch)`, `submit(ego_batch, gt_boxes)` with evaluation."""
+    """The pipeline over a mixed-modality scene, SceneGraph slots (FramePipeline.for_scene): `submit(ego_batch)` takes the
+    reference's collated `batch_data['ego']` and returns, pinned on the host, the boxes, scores and box count of frame
+    i - (depth - 1) when `postprocess_params` is given (`boxes[:count[0]]`), else its heads.  With `eval_thresholds` (and
+    `gt_capacity`, see SceneGraph) `submit(ego_batch, gt_boxes)` also takes the frame's GT, each frame is evaluated in its
+    graph, and `pipe.result_stat` collects the frames in the reference's format as they come back."""
+
+    def __init__(self, model, agent_modality_list, capacities, pairwise_shape, postprocess_params=None, device=None,
+                 compute_streams: int = 2, depth: int = 2, **graph_kwargs):
+        dev = device or next(model.parameters()).device
+        graphs = [SceneGraph(model, agent_modality_list, capacities, pairwise_shape, postprocess_params, device=dev,
+                             **graph_kwargs) for _ in range(max(2, int(depth)))]
+        self._start(graphs, dev, compute_streams, graphs[0].eval_thresholds)
 
     def submit(self, ego_batch, gt_boxes=None):
         return self._submit(ego_batch, gt_boxes)
@@ -826,7 +804,6 @@ class SceneStream(FramePipeline):
 
     def __init__(self, model, capacities, pairwise_shape, postprocess_params=None, depth: int = 2, max_graphs: int = 16,
                  voxel_limits=None, device=None, eval_thresholds=None, gt_capacity=None):
-        from . import ops
         dev = device or next(model.parameters()).device
         depth = max(1, int(depth))
         self.model, self.capacities, self.pairwise_shape = model, dict(capacities), tuple(pairwise_shape)
@@ -840,13 +817,13 @@ class SceneStream(FramePipeline):
         self.pools = [torch.cuda.graph_pool_handle() for _ in range(depth)]
         self.postprocess = [None] * depth
         if postprocess_params is not None:
-            H, W, A = _anchor_box(postprocess_params).shape[:3]
-            self.postprocess = [ops.PostprocessBuffers(H, W, A, 1000, dev) for _ in range(depth)]   # SceneGraph's `top`
+            H, W, A = _anchors(postprocess_params, "meta").shape[:3]
+            self.postprocess = [ops.PostprocessBuffers(H, W, A, TOP, dev) for _ in range(depth)]
         self.evals = [None] * depth
         if thresholds is not None:
-            self.evals = [FrameEval(1000, self.gt_capacity, dev) for _ in range(depth)]
+            self.evals = [FrameEval(TOP, self.gt_capacity, dev) for _ in range(depth)]
         self.lists = [None] * depth                             # the agent list of the frame that last used each slot
-        self._start(self.cache.slots, [None] * depth, dev, 2, thresholds)
+        self._start([None] * depth, dev, 2, thresholds)         # a slot's graphs are captured as frames need them
 
     def _capture(self, k, key):
         self.join(begin=False)          # the warm-up follows every frame in flight: slot k's last frame has left its buffers

@@ -286,11 +286,11 @@ class AgentShardedFrame:
     are captured and replayed alternately; the flag barrier of frame k+1 cannot pass before every rank has finished frame k."""
 
     def __init__(self, model, n_agents: int, rank: int, world: int, point_capacity: int, pairwise_shape, device=None,
-                 modality: str = "m1", shard_tail: bool = True, group=None, warmup: int = 2, comm: str = "auto"):
+                 modality: str = "m1", shard_tail: bool = True, group=None, comm: str = "auto"):
         _refuse_compressor(model)
         from . import ops
         from .engine import act_fmt
-        from ._lib import lib
+        from .graph import record, warm_up
         dev = device or next(model.parameters()).device
         self.model, self.rank, self.world, self.dev, self.group = model, rank, world, dev, group
         self.n_agents, self.m = n_agents, modality
@@ -360,22 +360,14 @@ class AgentShardedFrame:
         self.collectives_per_frame = self.exchanges_per_frame if comm == "nccl" else 0  # NCCL calls inside the frame
         self.side_stream = torch.cuda.Stream(device=dev)
         # warm-up (every side), then capture one graph per side
-        cap_stream = torch.cuda.Stream(device=dev)
-        cap_stream.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(cap_stream), torch.no_grad():
-            for _ in range(warmup):
-                for sd in self.sides:
-                    self._frame(sd)
-        torch.cuda.current_stream(dev).wait_stream(cap_stream)
-        torch.cuda.synchronize(dev)
+        warm_up(lambda: [self._frame(sd) for sd in self.sides], dev)
         if world > 1:
             dist.barrier(group=group)
-        l0 = lib.heal_launch_count()
+        kernels = 0
         for sd in self.sides:
-            sd["graph"] = torch.cuda.CUDAGraph()
-            with torch.no_grad(), torch.cuda.graph(sd["graph"], capture_error_mode="thread_local"):
-                sd["out"] = self._frame(sd)
-        self.kernels_per_replay = int(lib.heal_launch_count() - l0) // len(self.sides)
+            sd["graph"], sd["out"], k = record(lambda: self._frame(sd))
+            kernels += k
+        self.kernels_per_replay = kernels // len(self.sides)
         self.count = 0
         self.out = self.sides[0]["out"]
 

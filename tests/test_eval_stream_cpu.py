@@ -158,3 +158,14 @@ def test_gt_is_refused_without_evaluation_and_counted_in_the_copy():
     spec = scene_spec(SENSORS, ["m1", "m3"], CAPS)
     plain = check_scene(spec, ["m1", "m3"], LIMITS, b)
     assert check_scene(spec, ["m1", "m3"], LIMITS, b, _gt(7), 100) == plain + 7 * 96 + 4
+
+
+def test_decode_kwargs_of_the_scene_postprocess_block():
+    """decode_kwargs on the scenes' `postprocess:` block: the keyword arguments of the box decodes of VoxelPostprocessor,
+    SceneGraph and LateFusionGraph, with a dir head (the `dir_args` correction) and without one (no correction)."""
+    import scene_fixtures
+    from heal_b200.data_utils.post_processor.voxel_postprocessor import decode_kwargs
+    common = {"score_threshold": 0.2, "nms_threshold": 0.15, "order": "hwl", "gt_range": [-12.8, -12.8, -3, 12.8, 12.8, 1],
+              "top": 1000}
+    assert decode_kwargs(scene_fixtures.postprocess_params(), True) == {**common, "dir_offset": 0.7853, "num_bins": 2}
+    assert decode_kwargs(scene_fixtures.postprocess_params(), False) == {**common, "dir_offset": 0.0, "num_bins": 2}
