@@ -463,25 +463,49 @@ class LateFusionGraph:
     `capacities[m]`: for a lidar modality the point capacity of ALL its cavs together (raw clouds, `points` + `agent_offsets`; the
     live counts travel in the offsets), for a camera modality (cameras, image height, image width) per cav for normalised fp32
     images, or (cameras, frame height, frame width, torch.uint8) for raw uint8 (H0, W0, 3) frames, which the encoder resizes, crops
-    and normalises on the GPU.  The poses are inputs: replaying the graph for another scene uses that scene's transforms."""
+    and normalises on the GPU.  The poses are inputs: replaying the graph for another scene uses that scene's transforms.
+
+    Several graphs can share memory (LateFusionStream does so per pipeline slot), as SceneGraph's do: `inputs` are caller-owned
+    input buffers (`_input_buffers` of these capacities for as many or more cavs; the graph reads leading slices), `transforms` a
+    caller-owned (max_cav, 4, 4) fp32 device buffer of which the graph reads the leading (n, 4, 4), `postprocess_buffers`
+    caller-owned ops.PostprocessBuffers for (H * n or more, W, A, TOP), `eval_buffers` a caller-owned FrameEval, and `pool` the
+    private memory pool of the capture.  `voxel_limits[m]` overrides the encoder's {max_points_per_voxel, max_voxels} of a lidar
+    modality.  `staging`: pinned host tensors (`late_staging`) through which `load` sends the per-cav point offsets and poses
+    instead of pageable ones; the caller keeps them unwritten until the last load's copies are done."""
 
     CAMERA_KEYS = ("rots", "trans", "intrins", "post_rots", "post_trans")
 
     def __init__(self, model, modality_of_each_cav, capacities, postprocess_params, device=None, eval_thresholds=None,
-                 gt_capacity=None):
+                 gt_capacity=None, inputs=None, pool=None, postprocess_buffers=None, eval_buffers=None, transforms=None,
+                 voxel_limits=None, staging=None):
         dev = device or next(model.parameters()).device
         self.eval_thresholds, self.gt_capacity = eval_setup(postprocess_params, eval_thresholds, gt_capacity)
-        self.eval = FrameEval(TOP, self.gt_capacity, dev) if self.eval_thresholds is not None else None
+        self.eval = None
+        if self.eval_thresholds is not None:
+            self.eval = FrameEval(TOP, self.gt_capacity, dev) if eval_buffers is None else eval_buffers
         self.modalities = list(modality_of_each_cav)
         n = len(self.modalities)
         self.groups = {}
         for i, m in enumerate(self.modalities):
             self.groups.setdefault(m, []).append(i)
-        self.inputs = _input_buffers(scene_spec(model.sensor_type_dict, self.modalities, capacities), dev)
-        self.transforms = torch.eye(4, dtype=torch.float32, device=dev).repeat(n, 1, 1).contiguous()
+        self.spec = scene_spec(model.sensor_type_dict, self.modalities, capacities)
+        self.inputs = _input_buffers(self.spec, dev) if inputs is None else _input_views(self.spec, inputs)
+        self.voxel_limits = _voxel_limits(model, self.spec, voxel_limits)
+        for m, lim in self.voxel_limits.items():
+            self.inputs[m].update(lim)
+        if transforms is None:
+            self.transforms = torch.eye(4, dtype=torch.float32, device=dev).repeat(n, 1, 1).contiguous()
+        elif not isinstance(transforms, torch.Tensor) or transforms.dtype != torch.float32 or transforms.dim() != 3 \
+                or tuple(transforms.shape[1:]) != (4, 4) or transforms.shape[0] < n or not transforms.is_contiguous():
+            raise ValueError(f"transforms: a contiguous (max_cav >= {n}, 4, 4) fp32 buffer expected, got "
+                             f"{tuple(getattr(transforms, 'shape', ()))} {getattr(transforms, 'dtype', None)}")
+        else:
+            self.transforms = transforms[:n]
+        self.staging = staging
         self.anchors = _anchors(postprocess_params, dev)
         A = self.anchors.shape[2]
-        self.buffers = ops.PostprocessBuffers(self.anchors.shape[0] * n, self.anchors.shape[1], A, TOP, dev)
+        self.buffers = ops.PostprocessBuffers(self.anchors.shape[0] * n, self.anchors.shape[1], A, TOP, dev) \
+            if postprocess_buffers is None else postprocess_buffers
         decode = decode_kwargs(postprocess_params, True)       # the grouped heads always carry the dir channels
 
         def run():
@@ -492,7 +516,7 @@ class LateFusionGraph:
                 self.eval.run(post, self.eval_thresholds)
             return post
 
-        self.graph, self.out, self.kernels_per_replay = capture(run, dev)
+        self.graph, self.out, self.kernels_per_replay = capture(run, dev, pool)
 
     def load(self, batch_data, gt_boxes=None):
         """Copy a scene's inputs and cav -> ego transforms into the captured buffers (asynchronous copies on the current stream).
@@ -515,21 +539,121 @@ class LateFusionGraph:
                     buf["points"][total:total + pts.shape[0]].copy_(pts, non_blocking=True)
                     total += pts.shape[0]
                     offs.append(total)
-                buf["agent_offsets"].copy_(torch.tensor(offs, dtype=torch.int32), non_blocking=True)
+                if self.staging is None:
+                    buf["agent_offsets"].copy_(torch.tensor(offs, dtype=torch.int32), non_blocking=True)
+                else:
+                    host = self.staging["offsets"][m][:len(offs)]
+                    host.copy_(torch.tensor(offs, dtype=torch.int32))
+                    buf["agent_offsets"].copy_(host, non_blocking=True)
             else:
                 for j, i in enumerate(idx):
                     src = batch_data[cavs[i]][f"inputs_{m}"]
                     for k in ("imgs",) + self.CAMERA_KEYS:
                         raw = k == "imgs" and buf[k].dtype == torch.uint8         # raw frames (cams, H0, W0, 3) go in whole
                         buf[k][j].copy_(src[k][0][:, :3] if k == "imgs" and not raw else src[k][0], non_blocking=True)
-        T = torch.stack([torch.as_tensor(batch_data[c]['transformation_matrix']).reshape(4, 4).to(torch.float32) for c in cavs])
-        self.transforms.copy_(T, non_blocking=True)
+        mats = [torch.as_tensor(batch_data[c]['transformation_matrix']) for c in cavs]
+        if self.staging is None:
+            T = torch.stack([t.reshape(4, 4).to(torch.float32) for t in mats])
+            self.transforms.copy_(T, non_blocking=True)
+        else:
+            host = self.staging["transforms"][:len(cavs)]
+            for i, t in enumerate(mats):
+                if not t.is_cuda:
+                    host[i].copy_(t.reshape(4, 4))
+            self.transforms.copy_(host, non_blocking=True)
+            for i, t in enumerate(mats):                  # poses already on the device are copied there, after the staged ones
+                if t.is_cuda:
+                    self.transforms[i].copy_(t.reshape(4, 4), non_blocking=True)
         if self.eval is not None:
             self.eval.load(gt_boxes)
 
     def replay(self):
         self.graph.replay()
         return self.out
+
+    def results(self):
+        """The device tensors a frame's consumer reads, named as SceneGraph.results(): the boxes, scores and box count, with
+        evaluation also `eval` (EvalBuffers.packed at capacity TOP) and `gt_count`."""
+        out = {"boxes": self.buffers.boxes, "scores": self.buffers.scores, "count": self.buffers.count}
+        if self.eval is not None:
+            out.update(eval=self.eval.buffers.packed, gt_count=self.eval.gt_count)
+        return out
+
+
+def late_staging(capacities, sensor_type_dict, max_cav: int):
+    """Pinned host tensors through which LateFusionGraph.load sends a frame's per-cav point offsets ({m: (max_cav + 1,) int32} for
+    every lidar modality of `capacities`) and cav -> ego poses ((max_cav, 4, 4) fp32)."""
+    offsets = {m: torch.zeros((max_cav + 1,), dtype=torch.int32).pin_memory()
+               for m in capacities if sensor_type_dict.get(m) != "camera"}
+    return {"offsets": offsets, "transforms": torch.eye(4).repeat(max_cav, 1, 1).pin_memory()}
+
+
+def late_modalities(batch_data):
+    """The ordered modality of every cav of a late batch `{cav_id: cav_content}` (modality_of: its one `inputs_*` key)."""
+    from .models.heter_model_late import modality_of
+    return [modality_of(cav) for cav in batch_data.values()]
+
+
+def check_late_scene(sensor_type_dict, capacities, max_cav: int, voxel_limits, batch_data, gt_boxes=None, gt_capacity=None):
+    """Host-side checks of a late-fusion batch `{cav_id: cav_content}` (dataset order, ego first) against the captured graphs of
+    a LateFusionStream, before anything is copied and without reading the device: 1 to `max_cav` cavs, each of a modality the
+    model has (`sensor_type_dict`) and `capacities` gives; a lidar cav carries one raw cloud (`points` (P, 4) and `agent_offsets`
+    of length 2), not left for GPU filtering (`filter_points`), with the voxelisation limits `voxel_limits[m]` the graphs were
+    captured with when it names them, and the clouds of one modality fit its point capacity together; a camera cav's images
+    have the captured shape and kind (uint8 frames or fp32 images); every cav has a `transformation_matrix`; the GT passes
+    check_gt.  Raises ValueError; returns the bytes LateFusionGraph.load copies."""
+    mods = late_modalities(batch_data)
+    if not 0 < len(mods) <= max_cav:
+        raise ValueError(f"{len(mods)} cavs {mods}: the stream serves 1 to max_cav = {max_cav}")
+    spec = scene_spec(sensor_type_dict, mods, capacities)
+    nbytes = check_gt(gt_boxes, gt_capacity) + len(mods) * 64
+    points = dict.fromkeys(spec, 0)
+    for cav, m in zip(batch_data, mods):
+        content, sp = batch_data[cav], spec[m]
+        src = content[f"inputs_{m}"]
+        if "transformation_matrix" not in content:
+            raise ValueError(f"cav {cav!r}: no transformation_matrix")
+        if torch.as_tensor(content["transformation_matrix"]).numel() != 16:
+            raise ValueError(f"cav {cav!r}: transformation_matrix of {torch.as_tensor(content['transformation_matrix']).numel()} "
+                             "values, a 4 x 4 matrix expected")
+        if "lidar" in sp:
+            if "points" not in src or "agent_offsets" not in src:
+                raise ValueError(f"cav {cav!r} inputs_{m}: a raw cloud (points, agent_offsets) expected, not voxels")
+            if tuple(src["agent_offsets"].shape) != (2,):
+                raise ValueError(f"cav {cav!r} inputs_{m}: agent_offsets of shape {tuple(src['agent_offsets'].shape)}, a late-"
+                                 "fusion cav carries one cloud (2,)")
+            if src.get("filter_points"):
+                raise ValueError(f"cav {cav!r} inputs_{m}: clouds left for heal_mask_points (filter_on_gpu) are not served by a "
+                                 "captured frame; filter them in the dataset")
+            for key, v in voxel_limits[m].items():
+                if key in src and int(src[key]) != v:
+                    raise ValueError(f"cav {cav!r} inputs_{m}: {key} {int(src[key])}, the graph was captured with {v}")
+            pts = src["points"]
+            if pts.dim() != 2 or pts.shape[1] != 4:
+                raise ValueError(f"cav {cav!r} inputs_{m}: points of shape {tuple(pts.shape)}, (P, 4) expected")
+            points[m] += pts.shape[0]
+            if points[m] > sp["lidar"]:
+                raise ValueError(f"{m}: the scene's {sp['agents']} cavs have more points than the capacity {sp['lidar']}")
+            nbytes += pts.shape[0] * 16
+        else:
+            imgs = src["imgs"]
+            cams, h, w = sp["camera"]
+            if sp["raw"] != (imgs.dtype == torch.uint8):
+                raise ValueError(f"cav {cav!r} inputs_{m}: {'fp32 images' if sp['raw'] else 'raw uint8 frames'} for a graph "
+                                 f"captured with {'raw uint8 frames' if sp['raw'] else 'normalised fp32 images'}")
+            want = (1, cams, h, w, 3) if sp["raw"] else (1, cams, 3, h, w)
+            got = tuple(imgs.shape) if sp["raw"] else tuple(imgs.shape[:2]) + (3,) + tuple(imgs.shape[3:])
+            if imgs.dim() != 5 or got != want or (not sp["raw"] and imgs.shape[2] < 3):
+                raise ValueError(f"cav {cav!r} inputs_{m}: images of shape {tuple(imgs.shape)}, the graph was captured for {want}")
+            nbytes += cams * h * w * 3 * (1 if sp["raw"] else 4)
+            for key in LateFusionGraph.CAMERA_KEYS:
+                shape = (1, cams, 3, 3) if key in ("rots", "intrins", "post_rots") else (1, cams, 3)
+                v = src.get(key)
+                if v is None or tuple(v.shape) != shape:
+                    got = "missing" if v is None else f"of shape {tuple(v.shape)}"
+                    raise ValueError(f"cav {cav!r} inputs_{m}: {key} {got}, {shape} expected")
+                nbytes += v.numel() * 4
+    return nbytes + sum(4 * (sp["agents"] + 1) for sp in spec.values() if "lidar" in sp)
 
 
 def check_scene(spec, agent_modality_list, voxel_limits, ego_batch, gt_boxes=None, gt_capacity=None):
@@ -714,12 +838,14 @@ class ScenePipeline(FramePipeline):
 
 
 class SceneGraphCache:
-    """The host side of SceneStream: a frame's key and its refusals, and per pipeline slot the captured graphs by key, least
-    recently used first.  The key is the ordered `agent_modality_list` as a tuple (the ego first; the order is the fusion
-    order).  `capture(slot, key)` makes slot `slot`'s graph for `key`."""
+    """The host side of SceneStream and LateFusionStream: a frame's key and its refusals, and per pipeline slot the captured
+    graphs by key, least recently used first.  The key is an ordered modality list as a tuple: SceneStream's is the
+    `agent_modality_list` (the ego first; the order is the fusion order), LateFusionStream's every cav's modality in batch order
+    (the order decides NMS ties), which its `frame(batch, gt_boxes)` returns after check_late_scene.  `capture(slot, key)`
+    makes slot `slot`'s graph for `key`."""
 
     def __init__(self, sensor_type_dict, capacities, max_cav: int, voxel_limits, slots: int, max_graphs: int, capture,
-                 gt_capacity=None):
+                 gt_capacity=None, frame=None):
         if int(max_graphs) < 1:
             raise ValueError(f"max_graphs {max_graphs}: a slot keeps at least one graph")
         self.sensors, self.capacities = dict(sensor_type_dict), dict(capacities)
@@ -727,6 +853,7 @@ class SceneGraphCache:
         self.slots = [collections.OrderedDict() for _ in range(slots)]
         self.capture = capture
         self.gt_capacity = gt_capacity                          # None: the graphs do not evaluate
+        self.frame = self._scene_frame if frame is None else frame
         self.captures = 0
 
     def _spec(self, key):
@@ -741,9 +868,13 @@ class SceneGraphCache:
         self._spec(key)
         return key
 
-    def check(self, ego_batch, gt_boxes=None):
-        """The key of a collated `batch_data['ego']`, after the checks of `key` and of `check_scene` for the frame's own list
-        and GT (host only, nothing is copied)."""
+    def check(self, batch, gt_boxes=None):
+        """The key of a frame after its host checks (nothing is copied): `frame(batch, gt_boxes)` when the cache was made with
+        one (LateFusionStream), else those of a collated `batch_data['ego']`: the checks of `key` and of `check_scene` for the
+        frame's own list and GT."""
+        return self.frame(batch, gt_boxes)
+
+    def _scene_frame(self, ego_batch, gt_boxes):
         key = tuple(ego_batch["agent_modality_list"])
         check_scene(self._spec(key), key, self.voxel_limits, ego_batch, gt_boxes, self.gt_capacity)
         return key
@@ -848,6 +979,114 @@ class SceneStream(FramePipeline):
     def capture(self, agent_modality_list):
         """Capture the graphs of an agent list in every slot ahead of the stream (a list a slot already holds is kept)."""
         key = self.cache.key(agent_modality_list)
+        for k in range(self.depth):
+            self.cache.graph(k, key)
+
+    @property
+    def captures(self):
+        """Graph captures so far, recaptures after eviction included."""
+        return self.cache.captures
+
+    @property
+    def graphs_captured(self):
+        """Graphs the stream holds over all slots."""
+        return self.cache.graphs_captured
+
+
+def late_cache(sensor_type_dict, capacities, max_cav: int, voxel_limits, slots: int, max_graphs: int, capture, gt_capacity=None):
+    """LateFusionStream's SceneGraphCache: a frame is a late batch `{cav_id: cav_content}`, checked by check_late_scene and keyed
+    by its ordered cav modalities."""
+    def frame(batch_data, gt_boxes):
+        check_late_scene(sensor_type_dict, capacities, max_cav, voxel_limits, batch_data, gt_boxes, gt_capacity)
+        return tuple(late_modalities(batch_data))
+    return SceneGraphCache(sensor_type_dict, capacities, max_cav, voxel_limits, slots, max_graphs, capture, gt_capacity,
+                           frame=frame)
+
+
+class LateFusionStream(FramePipeline):
+    """A stream of late-fusion scenes whose cav list changes from frame to frame (the CAVs in range and their modalities, as
+    in a dataset's test split), for the single-agent models (HeterModelLate, HeterPyramidSingle), served through FramePipeline's
+    slots as SceneStream serves intermediate fusion.  `submit(batch_data)` takes what the late datasets collate
+    (`{cav_id: cav_content}` in dataset order, ego first, what the reference's `inference_late_fusion` loops over) and returns,
+    pinned on the host, frame i - (depth - 1): its boxes, scores and box count (`boxes[:count[0]]`) and its `modality_list`.
+
+        stream = LateFusionStream(model, {"m1": 400_000, "m2": (4, 600, 800, torch.uint8)}, max_cav=5,
+                                  postprocess_params=hypes["postprocess"], eval_thresholds=(0.3, 0.5, 0.7), gt_capacity=400)
+        for batch_data in data_loader:
+            gt = dataset.post_processor.generate_gt_bbx(batch_data)
+            res = stream.submit(batch_data, gt)                    # late; None while the pipeline fills
+            # no fusion: stream.submit({'ego': batch_data['ego']}, gt)
+            # single:    stream.submit({'ego': batch_data['ego']}, dataset.post_processor.generate_gt_bbx({'ego': batch_data['ego']}))
+        stream.drain()
+        eval_utils.eval_final_results(stream.result_stat, save_path, infer_info)
+
+    Each slot keeps one captured LateFusionGraph per ordered cav-modality list, so a frame's boxes are bit for bit those of a
+    LateFusionGraph captured for its list alone.  A list new to a slot is captured inside `submit` (a device synchronise and two
+    eager warm-up frames); `capture(modality_list)` does it ahead.  Above `max_graphs` graphs in a slot the least recently used
+    one is dropped (and recaptured if its list comes back).  A frame that cannot be served raises ValueError on the host before
+    anything is copied (check_late_scene).  `capacities` follows LateFusionGraph for every modality the stream may see; a lidar
+    capacity holds the clouds of all its cavs in one frame.  `max_cav` is at most 16, the limit of heal_box_decode_nms_late.
+
+    With `eval_thresholds` every graph ends in heal_eval_tp_fp_counted: `submit(batch_data, gt_boxes)` takes the frame's GT
+    ((G, 8, 3) fp32 corners, the reference's `post_processor.generate_gt_bbx(batch_data)`: the union of every cav's objects, so
+    `gt_capacity`, by default `postprocess_params['max_num']`, may need to be larger), and `stream.result_stat` gains each
+    frame once, in frame order, in the reference's format, as in SceneStream.
+
+    Inputs and GT are device or pinned host tensors; the per-cav point offsets and host-side poses go through the slot's pinned
+    staging tensors, so `submit` issues no pageable copy and reads nothing back for a list its slot holds.  Memory: the graphs
+    of slot k are captured into one private pool, read slot k's one set of input buffers (every modality at its capacity, for
+    max_cav cavs) and one (max_cav, 4, 4) transforms buffer, and write slot k's one set of post-processing (sized for max_cav
+    cavs) and evaluation buffers, which lie outside the pool.  Graphs of one slot never run at once, so they share their
+    scratch: a frame's device results are valid only until its slot's next replay; the host results are valid until the slot's
+    next copy-out, `depth` submits later, as in FramePipeline."""
+
+    def __init__(self, model, capacities, max_cav: int, postprocess_params, depth: int = 2, max_graphs: int = 16,
+                 voxel_limits=None, device=None, eval_thresholds=None, gt_capacity=None):
+        if not _count(max_cav) or max_cav > 16:
+            raise ValueError(f"max_cav {max_cav!r}: 1 to 16 cavs, the limit of heal_box_decode_nms_late")
+        dev = device or next(model.parameters()).device
+        depth = max(1, int(depth))
+        self.model, self.capacities, self.max_cav = model, dict(capacities), int(max_cav)
+        self.postprocess_params, self.voxel_limits = postprocess_params, voxel_limits
+        thresholds, self.gt_capacity = eval_setup(postprocess_params, eval_thresholds, gt_capacity)
+        spec = scene_spec(model.sensor_type_dict, list(self.capacities), self.capacities)
+        self.cache = late_cache(model.sensor_type_dict, self.capacities, self.max_cav, _voxel_limits(model, spec, voxel_limits),
+                                depth, max_graphs, self._capture, self.gt_capacity)
+        self.inputs = [_input_buffers({m: dict(sp, agents=self.max_cav) for m, sp in spec.items()}, dev) for _ in range(depth)]
+        self.transforms = [torch.eye(4, dtype=torch.float32, device=dev).repeat(self.max_cav, 1, 1) for _ in range(depth)]
+        self.staging = [late_staging(self.capacities, model.sensor_type_dict, self.max_cav) for _ in range(depth)]
+        self.pools = [torch.cuda.graph_pool_handle() for _ in range(depth)]
+        H, W, A = _anchors(postprocess_params, "meta").shape[:3]
+        self.postprocess = [ops.PostprocessBuffers(H * self.max_cav, W, A, TOP, dev) for _ in range(depth)]
+        self.evals = [None] * depth
+        if thresholds is not None:
+            self.evals = [FrameEval(TOP, self.gt_capacity, dev) for _ in range(depth)]
+        self.lists = [None] * depth                             # the modality list of the frame that last used each slot
+        self._start([None] * depth, dev, 2, thresholds)
+
+    def _capture(self, k, key):
+        self.join(begin=False)          # the warm-up follows every frame in flight: slot k's last frame has left its buffers
+        return LateFusionGraph(self.model, list(key), self.capacities, self.postprocess_params, device=self.dev,
+                               eval_thresholds=self.eval_thresholds, gt_capacity=self.gt_capacity, inputs=self.inputs[k],
+                               pool=self.pools[k], postprocess_buffers=self.postprocess[k], eval_buffers=self.evals[k],
+                               transforms=self.transforms[k], voxel_limits=self.voxel_limits, staging=self.staging[k])
+
+    def _slot(self, k, batch_data, gt_boxes=None):
+        key = self.cache.check(batch_data, gt_boxes)
+        g = self.cache.graph(k, key)
+        self.lists[k] = key
+        self._bind(k, g.results())
+        return g
+
+    def _result(self, k):
+        return {**self.host_out[k], "modality_list": list(self.lists[k])}
+
+    def submit(self, batch_data, gt_boxes=None):
+        return self._submit(batch_data, gt_boxes)
+
+    def capture(self, modality_list):
+        """Capture the graphs of a cav-modality list in every slot ahead of the stream (a list a slot already holds is kept)."""
+        key = self.cache.key(modality_list)
         for k in range(self.depth):
             self.cache.graph(k, key)
 

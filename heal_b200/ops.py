@@ -1705,7 +1705,8 @@ def box_decode_nms_late(cls_preds, reg_preds, dir_preds, anchors: torch.Tensor, 
     """Late fusion of one scene on the GPU with no host sync and no host-side pose: heads of every cav as one batched map each
     ((n_cav, A, H, W) / (n_cav, 7A, H, W) / (n_cav, A*bins, H, W) or None; or f32 Acts, read from channel `coffsets`), one shared
     anchor grid (H, W, A, 7) and DEVICE transforms (n_cav, 4, 4) fp32.  Same boxes, order and scores as box_decode_nms_multi
-    over the same cavs in batch order."""
+    over the same cavs in batch order.  `buffers` may be made for more cavs (H * max_cav rows) than the call has, so that the
+    graphs of several cav lists share one set (LateFusionStream)."""
     c, r = _late_heads(cls_preds, "cls_preds"), _late_heads(reg_preds, "reg_preds")
     d = _late_heads(dir_preds, "dir_preds") if dir_preds is not None else None
     oc, orr, od = (int(v) for v in coffsets)
@@ -1730,8 +1731,9 @@ def box_decode_nms_late(cls_preds, reg_preds, dir_preds, anchors: torch.Tensor, 
         raise ValueError(f"box_decode_nms_late: transforms must be a contiguous ({n}, 4, 4) fp32 CUDA tensor")
     if buffers is None:
         buffers = PostprocessBuffers(H * n, W, A, top, anchors.device)
-    if (buffers.H, buffers.W, buffers.A, buffers.top) != (H * n, W, A, top):
-        raise ValueError("box_decode_nms_late: buffers were made for another geometry")
+    if (buffers.W, buffers.A, buffers.top) != (W, A, top) or buffers.H < H * n:     # the C ABI checks the workspace bytes too
+        raise ValueError(f"box_decode_nms_late: buffers were made for another geometry: H {buffers.H}, W {buffers.W}, A "
+                         f"{buffers.A}, top {buffers.top}; {n} cavs need H >= {H * n}, W {W}, A {A}, top {top}")
     rng = _box_range_f32(gt_range) if gt_range is not None else None
     with _Prof("box_decode_nms", 0):
         _call("heal_box_decode_nms_late", c.view(oc), r.view(orr), d.view(od) if d is not None else None, _p(anchors),
